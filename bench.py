@@ -39,10 +39,10 @@ sys.path.insert(0, ROOT)
 
 FIDUCIAL_LEN = 0.14
 DEPTH = int(os.environ.get("FID_BENCH_DEPTH", "2"))            # batches in flight (each takes FRAMES/SLOT of the library's FID_SLOTS chunk slots)
-HBM_FALLBACK_GBS = 6650.0
+HBM_FALLBACK_GBS = 3350.0  # H100 SXM data sheet (HBM3), used when no measured copy bandwidth is at hand
 REALIZATIONS = 8   # noise realisations per marker layout of the synthetic stream (a layout costs 0.8 s of numpy to render)
-# BASELINE.json configs that are frame streams: frames per step per GPU (each step's frames are distinct and >> 126 MB L2),
-# frames per in-flight chunk inside the library, description.  The driver's default is C2 (the config the metric is quoted on).
+# BASELINE.json configs that are frame streams: frames per step per GPU (each step's frames are distinct and >> the 50 MB L2 of an H100),
+# frames per in-flight chunk inside the library, description.  The default is C2 (the config the metric is quoted on).
 WORKLOADS = {
     "C2": dict(frames=128, slot=64, desc="C2: 1920x1080 BGR8 stream, 16 markers/frame, DICT_6X6_250, detect+pose+map update"),
     "C3": dict(frames=256, slot=128, desc="C3: 1280x720 BGR8 camera stream per GPU, 8 markers/frame, DICT_5X5_250, detect+pose+map update, merged map by NCCL all-gather"),
@@ -149,7 +149,7 @@ def rank_info():
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons during the timed region."""
 
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -197,7 +197,7 @@ def measured_hbm_peak():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured copy bandwidth)"
     except Exception:
-        return HBM_FALLBACK_GBS, "fallback 6.65 TB/s (B200_PROFILING.md)"
+        return HBM_FALLBACK_GBS, "H100 SXM data sheet 3.35 TB/s (not a measured figure)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -229,8 +229,8 @@ class CpuArm:
     """The reference's CPU path on a bounded sample, in both modes (BASELINE.md section 3.5):
     reference mode  = one process, OpenCV threads = all cores (what the single-threaded node does);
     throughput mode = single-threaded worker processes, frames round-robin: one per logical core, one per
-                      physical core, and -- under a cgroup CPU quota -- one and two per core of the quota (half of them on an SMT box -- the detector is memory bound and ran 30 % faster
-                      that way on the 128-thread host of the B200 box).
+                      physical core, and -- under a cgroup CPU quota -- one and two per core of the quota (half of them on an SMT box: the detector is memory bound
+                      and may run faster that way).
     The worker pools are spawned once (spawn, so OpenCV's thread pool is never forked) and reused by every
     measure() call: --impl reference times K steps without paying K pool start-ups."""
 
@@ -408,6 +408,36 @@ def parity_gate(frames, idx, out, dict_id, K, D, maxm):
             "bars": "ids identical and in identical order; corners, tvec, quaternion <= 1e-3 vs oracle/aruco_oracle.py (cv2) on frames of the timed batch"}
 
 
+def map_array(entries):
+    """Map entries as rows: id, num_obs, x, y, z, rx, ry, rz, variance."""
+    return np.array([[e.fiducial_id, e.num_obs, e.x, e.y, e.z, e.rx, e.ry, e.rz, e.variance] for e in entries], np.float64).reshape(-1, 9)
+
+
+def dump_outputs(dirname, out, map_entries):
+    """--dump-outputs: the results of the last timed step as a caller of the detect+pose+map path receives them -- per frame of
+    the batch the marker count, ids, corners and transforms (slots past a frame's count zeroed), and the camera map after the
+    step -- in float32 / float64, so that two builds can be compared output for output on the same seeded stream."""
+    from fiducials_b200.node import MAXM, FiducialSlam
+
+    os.makedirs(dirname, exist_ok=True)
+    counts, ids, corners, tfs = out
+    n = len(counts)
+    valid = np.arange(MAXM)[None, :] < counts[:, None]
+    tf = np.frombuffer(tfs, dtype=FiducialSlam.TRANSFORM_DTYPE, count=n * MAXM).reshape(n, MAXM)
+    arrays = {
+        "counts": counts.astype(np.float64),
+        "ids": np.where(valid, ids, 0).astype(np.float64),
+        "corners": np.where(valid[:, :, None, None], corners, 0).astype(np.float32),
+    }
+    for name in ("translation", "rotation", "rvec"):
+        arrays[name] = np.where(valid[:, :, None], tf[name], 0).astype(np.float64)
+    for name in ("image_error", "object_error", "fiducial_area"):
+        arrays[name] = np.where(valid, tf[name], 0).astype(np.float64)
+    arrays["map"] = map_array(map_entries)
+    for name, a in arrays.items():
+        np.save(os.path.join(dirname, name + ".npy"), a)
+
+
 # ------------------------------------------------------------------------------------------------
 # our arm
 # ------------------------------------------------------------------------------------------------
@@ -522,6 +552,8 @@ def run_gpu_arm(args):
     stage_ms = det.last_stage_ms()  # stages of the last batch call (nf frames)
     counters = det.last_counters()
     last_out = outs[(args.steps - 1) & 3]
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_out, slam.entries(0))
     e2e_s, e2e_wall, _, _ = timed(False, args.steps)
     clocks = sampler.stop()
     n_merged = len(slam.merged_entries())
@@ -567,14 +599,6 @@ def run_gpu_arm(args):
         n_launch_thr = (nf + slot_frames - 1) // slot_frames
         thr_pipe_ms = stage_ms["threshold"] / n_launch_thr
         total_stage = sum(v for k, v in stage_ms.items() if k not in ("h2d", "d2h") and not k.startswith("walk_r"))
-        traffic, traffic_src = None, None
-        try:  # DRAM bytes of the kernel from the committed ncu --set full capture of this round (per frame, scaled to this launch)
-            tj = json.load(open(os.path.join(ROOT, "profiles", "r02_threshold_traffic.json")))
-            if tj.get("workload") == WORKLOAD:
-                traffic = float(tj["dram_bytes_per_frame"]) * chunk
-                traffic_src = "profiles/r02_threshold_traffic.json (ncu --set full capture of the same kernel and workload; not re-measured by this run)"
-        except Exception:
-            pass
         roofline = {
             "bound": "hbm",
             "kernel": ("k_threshold_mma (BGR->gray + 13 adaptive thresholds on the int8 tensor cores + halo tiles + start cracks, one launch)" if os.environ.get("FID_THRESH") == "mma" else "k_threshold<FAST> (threshold stage in one launch: BGR->gray fused into the region load, summed-area table in shared memory, 13 thresholds, halo tiles + start cracks)"),
@@ -582,8 +606,8 @@ def run_gpu_arm(args):
             "peak": peak,
             "unit": "GB/s",
             "frac": achieved / peak,
-            "traffic": traffic,
-            "traffic_source": traffic_src,
+            "traffic": None,
+            "traffic_source": "not measured",
             "peak_source": peak_src + "; kernel timed alone -> burst figure",
             "algorithmic_bytes_per_launch": algo_bytes,
             "frames_per_launch": chunk,
@@ -620,7 +644,7 @@ def run_gpu_arm(args):
             "config": {
                 "workload": workload_string(WORKLOAD),
                 "frames_per_step_per_gpu": nf,
-                "l2": "inputs larger than L2 (%d MB of distinct frames per step vs 126 MB L2)" % (frames.nbytes // 2**20),
+                "l2": "inputs larger than L2 (%d MB of distinct frames per step vs 50 MB L2)" % (frames.nbytes // 2**20),
                 "parallelism": ("one camera stream per GPU, no collective on detect/pose; per step the local map tables are exported, all-gathered (NCCL) and merged on the "
                                 "map's CUDA stream without blocking the host") if world > 1 else "1 GPU",
                 "markers_found_per_step": n_markers_found // max(1, args.steps),
@@ -728,6 +752,9 @@ def run_c5(args, reference):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     dt = float(t[0])
     ents = slam.entries(0)
+    if args.dump_outputs and rank == 0:  # the map the last timed step folded
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "map.npy"), map_array(ents))
     # the north-star's batched SE(3) Gauss-Newton over the same observations (fid_map_refine; new, parity unpinned): cost, the
     # reference's plane-fit metric (fiducial_slam/scripts/fit_plane.py; the synthetic ceiling is the plane z = 2.5) and wall time
     refine = None
@@ -784,7 +811,9 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--workload", default="C2", choices=["C2", "C3", "C4", "C5"], help="BASELINE.json config (the driver's default, C2, is the one the metric is quoted on)")
+    ap.add_argument("--workload", default="C2", choices=["C2", "C3", "C4", "C5"], help="BASELINE.json config (the default, C2, is the one the metric is quoted on)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one returned (detections, poses, camera map) as DIR/<name>.npy")
     args = ap.parse_args()
     global WORKLOAD
     WORKLOAD = args.workload

@@ -1,4 +1,4 @@
-"""In-tree build of libfiducials_b200.so (nvcc, sm_100a only).  Used by __graft_entry__.build()."""
+"""In-tree build of libfiducials_b200.so (nvcc, sm_90a only).  Used by __graft_entry__.build()."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,7 @@ OUT = os.path.join(HERE, "libfiducials_b200.so")
 SOURCES = ["fid_api.cu", "fid_map.cu", "fid_map_refine.cu", "fid_jpeg.cu"]
 # --fmad=false: OpenCV's float32/float64 arithmetic (cornerSubPix, perimeters, the LM trajectory) is
 # compiled without FMA contraction on x86-64; contracting here would change iteration counts.
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "--fmad=false", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "--fmad=false", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
 
 def _newest_source():

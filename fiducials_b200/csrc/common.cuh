@@ -1,7 +1,7 @@
 // Common definitions for the fiducials_b200 device code.
 //
 // All per-element logic of the pipeline lives in FID_HD functions so that the *same source* is
-// compiled (a) by nvcc into the sm_100a kernels of libfiducials_b200.so (the product) and (b) by
+// compiled (a) by nvcc into the sm_90a kernels of libfiducials_b200.so (the product) and (b) by
 // g++ into tests/hostsim (a CPU unit-test harness for the device functions; never linked into the
 // product library, never reachable from the C-ABI).
 #pragma once

@@ -72,7 +72,7 @@ struct Slot {
 
 struct fid_detector {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;  // H100 SXM; replaced by the device's count in fid_create
     fid_params params{};
     DevParams P{};
     int max_w = 0, max_h = 0, max_batch = 0;

@@ -1,4 +1,4 @@
-// CUDA kernels, contour half of the per-frame pipeline (sm_100a); the threshold stage that feeds it
+// CUDA kernels, contour half of the per-frame pipeline (sm_90a); the threshold stage that feeds it
 // is in kernels_threshold.cuh:
 //   k_walk          one thread per start crack / suspended walk, in rounds: round 0 one-directional, later
 //                   rounds bidirectional; canonical test, contour length, emission segments      (A.3b)
@@ -6,7 +6,7 @@
 //   k_approx_warp   one warp per contour (<= 1024 points): approxPolyDP + quad filters             (A.4)
 //   k_approx        one block per longer contour
 // All kernels take a batch of frames (blockIdx.z / queue entries carry the frame index) so that a
-// launch has enough independent work to fill 148 SMs.
+// launch has enough independent work to fill the 132 SMs of an H100.
 #pragma once
 #include <cuda_runtime.h>
 

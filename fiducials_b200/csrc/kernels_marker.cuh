@@ -1,4 +1,4 @@
-// CUDA kernels, back half of the per-frame pipeline (sm_100a):
+// CUDA kernels, back half of the per-frame pipeline (sm_90a):
 //   k_sort_group  one block per frame: clockwise fix, stable descending-perimeter order, pairwise
 //                 "too close" matrix, OpenCV's order-dependent grouping                  (SURVEY A.5)
 //   k_identify_first / k_identify_retry   one warp per selected candidate, one block per failed first attempt: perspective removal, Otsu, cell votes, border

@@ -1,4 +1,4 @@
-// CUDA kernels, threshold stage (sm_100a):
+// CUDA kernels, threshold stage (sm_90a):
 //   k_gray       BGR8 -> gray (cv::cvtColor BGR2GRAY, 15-bit fixed point, SURVEY A.1); 4 pixels per
 //                thread, 12-byte vector loads / 4-byte store
 //   k_threshold  frame (BGR8/RGB8/MONO8; cvtColor fused into the load) -> n_scales adaptive-threshold planes (SURVEY A.2), written directly as the

@@ -1,4 +1,4 @@
-// Threshold stage on the 5th-generation tensor cores (sm_100a): tcgen05.mma kind::i8 + TMEM + TMA.
+// Threshold stage on the Hopper tensor cores (sm_90a): wgmma u8 x u8 -> s32 + TMA + mbarrier.
 //
 // Replaces the 13 cv::adaptiveThreshold passes inside cv::aruco::detectMarkers
 // (aruco_detect/src/aruco_detect.cpp:350, windows :691-693) and the cvtColor before them, for the
@@ -8,25 +8,31 @@
 //   box sum S_r(x,y) = sum_{dy=-r..r} H_r(x, y+dy),   H_r(x,y') = sum_{dx=-r..r} g(x+dx, y')
 //
 // * H_r for a whole tile is ONE banded matrix product  D[x][y'] = sum_i A_r[x][i] * G[y'][i]
-//   (A_r = 0/1 band, u8; G = gray region, u8; exact s32 accumulators in TMEM): tcgen05.mma
-//   cta_group::1 kind::i8, M = 128 output columns, N = 112 region rows, K = 192 region columns.
-//   With the lanes in REVERSED column order the band matrix is a Hankel matrix (entry depends on
-//   lane + i only), so its 8x16-byte core matrices are shared along the anti-diagonals: a whole
-//   128 x 192 operand is a 38-core-matrix (4.9 KB) table addressed with SBO = 128 B, LBO = 256 B
-//   (tools/probe_umma.cu validates the aliasing on hardware).  The centre pixel g(x,y) comes from the
-//   same machinery with r = 0.
-// * The vertical part is a running sum in registers: an epilogue thread owns one column (one TMEM
-//   lane), streams H_r(x, .) out of TMEM with tcgen05.ld (leading and trailing edge of the window)
-//   and spends three instructions per pixel and scale:  D = g*(-k^2) + V  (IMAD),  shift the sign
-//   of D into the column word (SHF),  V += lead - trail (IADD3).   [the table kernel: 11.5, 4 of them LDS]
+//   (A_r = 0/1 band, u8; G = gray region, u8; exact s32 accumulators in registers):
+//   wgmma.mma_async m64n112k32 .s32.u8.u8, two warpgroups of M = 64 output columns each, N = 112
+//   region rows, K = 192 region columns (the 4 k-steps that cover the band of the warpgroup's columns).
+//   With the rows in REVERSED column order the band matrix is a Hankel matrix (entry depends on
+//   row + i only), so its 8x16-byte core matrices are shared along the anti-diagonals: a whole
+//   128 x 192 operand is a 38-core-matrix (4.9 KB) table addressed with SBO = 128 B, LBO = 256 B;
+//   the second warpgroup starts 8 core matrices (1 KB) into it.
+// * The vertical part is a running sum in registers.  Each warpgroup parks its accumulators in shared
+//   memory as u16 (H_r <= 51 * 255), one column per 114-entry row; an epilogue thread then owns one
+//   column and one 32-row band, streams H_r(x, .) back (leading and trailing edge of the window)
+//   and spends three integer operations per pixel and scale:  D = g*(-k^2) + V,  the sign of D into
+//   the column word,  V += lead - trail.  The wgmma chain of the next scale is issued before this loop but
+//   completes before it starts: it is issued on a conditional path, and ptxas waits for it where the paths
+//   join.  Keeping it in flight across the loop (last scale peeled off, issue unconditional) measured 2.5 %
+//   slower on H100, the larger code costing more than the overlap gains.  Two parking buffers per
+//   warpgroup let a scale be parked while slower threads still read the previous one.  The centre pixels g
+//   come straight from the gray tile.
 // * BGR tiles are staged by TMA (cp.async.bulk.tensor.3d over a u32 view of the BGR rows, 16-row
 //   bands, 4-deep mbarrier ring) and converted to gray in shared memory -- no gray plane in HBM.
 //   Tiles whose region leaves the image take a clamping global-load path (replicate border, which
 //   TMA's zero fill cannot express): 22 % of the tiles at 1080p.
-// * One persistent CTA per SM, warp specialised: warp 0 TMA producer, warp 1 MMA issuer, warps 4-7
-//   BGR->gray converters (they write the MMA's B operand), warps 8-15 epilogue (two groups of four
-//   alternate over the scales, each ping-ponging on two TMEM accumulators) which leave column words in shared
-//   memory; warps 16-19 take them from there, one warp per two 30x30 halo tiles: 32x32 bit transposes (column words -> row words), the 128-byte tile
+// * One persistent CTA per SM, warp specialised: warp 0 TMA producer, warps 4-7 BGR->gray converters
+//   (they write the MMA's B operand), warps 8-15 the two MMA + epilogue warpgroups, which leave column
+//   words in shared memory; the converter warps take them from there while the next tile runs, one
+//   warp per two 30x30 halo tiles: 32x32 bit transposes (column words -> row words), the 128-byte tile
 //   stores and the start cracks of the border walk, exactly as in kernels_threshold.cuh.
 // Algorithmic HBM bytes per frame (SURVEY 8d): 3*W*H in + 13*W*H/8 out.
 #pragma once
@@ -39,9 +45,8 @@
 
 namespace fid {
 
-#define TM_THREADS 512       // 4 warpgroups: {TMA, MMA, 2 idle}, 4 converters, 2 x 4 epilogue
+#define TM_THREADS 512       // 4 warpgroups: {TMA, 3 idle}, 4 converters, 2 x 4 MMA + epilogue
 #define TM_WARP_TMA 0
-#define TM_WARP_MMA 1
 #define TM_WARP_CONV0 4
 #define TM_NCONV 4
 #define TM_WARP_EPI0 8
@@ -58,8 +63,8 @@ static_assert(TM_REGS_CTRL + TM_REGS_CONV + 2 * TM_REGS_EPI <= 4 * 128, "setmaxn
 #define TM_B_LBO (TM_N * 16)          // row-contiguous B tile: (n, i) at (i/16)*TM_B_LBO + n*16 + i%16
 #define TM_B_BYTES (12 * TM_B_LBO)    // 21504
 #define TM_A_BYTES (38 * 128)         // one Hankel table
-#define TM_NTAB 14                    // r = 0 (centre pixel) and the 13 window radii
-#define TM_C0 154                     // band: A[lane][i] = |i + lane - 154| <= r   (lane = 127 - (x - (X0-1)), i = x - (X0-28))
+#define TM_NTAB 13                    // the 13 window radii
+#define TM_C0 154                     // band: A[m][i] = |i + m - 154| <= r   (m = 127 - (x - (X0-1)), i = x - (X0-28))
 #define TM_BOXW 148                   // u32 per staged BGR row: 592 B >= 3*(180 + 12); 148 mod 32 = 20 keeps the converters' loads conflict-free
 #define TM_BOXH 16
 #define TM_NBANDS 7
@@ -71,17 +76,17 @@ static_assert(TM_REGS_CTRL + TM_REGS_CONV + 2 * TM_REGS_EPI <= 4 * 128, "setmaxn
 #define TM_OFF_B (TM_OFF_A + TM_NTAB * TM_A_BYTES)
 #define TM_OFF_STAGE (TM_OFF_B + 2 * TM_B_BYTES)
 #define TM_OFF_COLW (TM_OFF_STAGE + TM_NSTAGES * TM_STAGE_STRIDE)
-#define TM_OFF_BAR (TM_OFF_COLW + 2 * TM_COLW_WORDS * 4)
+// parked accumulators: per warpgroup two buffers of 64 columns x TM_DSTRIDE u16 (region rows 0..111).  57 words per
+// column (odd): the 32 columns a warp reads at one row fall in 32 different banks
+#define TM_DSTRIDE 114
+#define TM_D_BYTES (64 * TM_DSTRIDE * 2)
+#define TM_OFF_D (TM_OFF_COLW + 2 * TM_COLW_WORDS * 4)
+#define TM_OFF_BAR (TM_OFF_D + 4 * TM_D_BYTES)
 #define TM_SMEM_BYTES (TM_OFF_BAR + 256)
+static_assert(TM_SMEM_BYTES <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 
 // barrier indices (uint64 each)
-enum { TMB_STAGE_FULL = 0, TMB_STAGE_EMPTY = 4, TMB_B_FULL = 8, TMB_B_EMPTY = 10, TMB_G_FULL = 12, TMB_G_EMPTY = 13, TMB_D_FULL = 14, TMB_D_EMPTY = 18, TMB_COLW_FULL = 22, TMB_COLW_EMPTY = 24, TMB_COUNT = 26 };
-// TMEM (512 columns): four H accumulators of 112 columns (each epilogue group ping-pongs on two of them, so the MMAs of
-// its next scale run under its current one) and the 64-column centre-pixel accumulator (region rows 25..88).
-#define TM_DCOLS 112
-#define TM_GCOL (4 * TM_DCOLS)
-#define TM_GROW0 25
-#define TM_GN 64
+enum { TMB_STAGE_FULL = 0, TMB_STAGE_EMPTY = 4, TMB_B_FULL = 8, TMB_B_EMPTY = 10, TMB_COLW_FULL = 12, TMB_COLW_EMPTY = 14, TMB_COUNT = 16 };
 
 struct ThreshMmaArgs {
     const uint8_t* src;  // frames as given (cv_bridge encoding `enc`), device memory
@@ -126,34 +131,41 @@ __device__ __forceinline__ void tm_mbar_expect_tx(uint64_t* b, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(tm_smem(b)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ uint64_t tm_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    // shared-memory matrix descriptor, K-major, no swizzle: start >> 4 [0,14), LBO >> 4 [16,30), SBO >> 4 [32,46), version 1 at [46,48)
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46);
+    // wgmma shared-memory matrix descriptor, K-major, no swizzle: start >> 4 [0,14), LBO >> 4 [16,30), SBO >> 4 [32,46),
+    // base offset 0, layout type 0 (no swizzle) at [62,64)
+    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);
 }
-__device__ __forceinline__ void tm_mma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-                 : "memory");
+// D (64 x 112, s32) (+)= A (64 x 32, u8, shared) * B (112 x 32, u8, shared)^T, issued by a whole warpgroup.  Fragment: warp w of the
+// warpgroup, lane l holds rows 16 w + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1):  d[4 j + 2 h + e] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + e]
+__device__ __forceinline__ void tm_wgmma(uint32_t (&d)[56], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n112k32.s32.u8.u8 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,"
+        "%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55}, %56, %57, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]),
+          "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]),
+          "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]),
+          "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]),
+          "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tm_commit(uint64_t* b) { asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(tm_smem(b)) : "memory"); }
-__device__ __forceinline__ void tm_ld16(uint32_t taddr, uint32_t* v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]),
-                   "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                 : "r"(taddr));
+__device__ __forceinline__ void tm_wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void tm_wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void tm_wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accesses of the accumulator registers across wgmma issue / wait
+__device__ __forceinline__ void tm_wg_fence_regs(uint32_t (&d)[56]) {
+#pragma unroll
+    for (int i = 0; i < 56; i++) asm volatile("" : "+r"(d[i])::"memory");
 }
-__device__ __forceinline__ void tm_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tm_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tm_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void tm_fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// one lane of a converged warp (the same one every time); the single-thread instructions (TMA, tcgen05.mma, tcgen05.commit) are
-// issued under it while the loop around them stays warp-uniform, so addresses and descriptors live in uniform registers
+// one lane of a converged warp (the same one every time); the single-thread TMA instructions are issued under it while the
+// loop around them stays warp-uniform, so addresses live in uniform registers
 __device__ __forceinline__ bool tm_elect() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
     return pred != 0;
 }
-// accumulator slot / phase of global scale index j = tile_iteration * 13 + scale: group j & 1 owns slots 2 (j & 1) and 2 (j & 1) + 1
-__device__ __forceinline__ uint32_t tm_slot_of(uint32_t j) { return 2u * (j & 1u) + ((j >> 1) & 1u); }
-__device__ __forceinline__ uint32_t tm_slot_use(uint32_t j) { return j >> 2; }
 template <int N>
 __device__ __forceinline__ void tm_regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N>
@@ -178,8 +190,8 @@ __device__ __forceinline__ void tm_tile_coords(const ThreshMmaArgs& a, int t, in
     *by = rem / a.tiles_x;
     *bx = rem - *by * a.tiles_x;
 }
-// TMA wants the box to start on a 16-byte boundary of the row (a start that is only 4-byte aligned is an illegal
-// instruction on sm_100a, tools/probe_tma2.cu): 3 bytes per pixel -> the box starts `tm_box_lead` pixels left of the
+// The box starts on a 16-byte boundary of the row (TMA is only specified for 16-byte aligned boxes of this u32 view):
+// 3 bytes per pixel -> the box starts `tm_box_lead` pixels left of the
 // region, at a column that is a multiple of 16 (X0 - 28 = 120 bx - 28 = 8 bx + 4 mod 16).
 __device__ __forceinline__ int tm_box_lead(int bx) { return (bx & 1) ? 12 : 4; }
 // region of the tile lies inside the image: TMA (zero fill outside) may stage it
@@ -269,6 +281,22 @@ __device__ __forceinline__ unsigned int start_reserve(StartAlloc& al, unsigned i
     return pos;
 }
 
+// H_r of scale s for the warpgroup's 64 columns xm_lo .. xm_lo + 63 (region columns i = xm + 27 - r .. xm + 27 + r, r <= 25):
+// k-steps 0..3 for xm_lo = 0, 2..5 for xm_lo = 64 cover that band for every scale (steps outside it add zeros), so the chain
+// has a fixed length.  Asynchronous: tm_wg_wait0() before the accumulators are read.
+__device__ __forceinline__ void tm_issue_scale(uint32_t (&acc)[56], uint64_t adesc0, uint64_t bdesc, int s, int xm_lo) {
+    const int kk_lo = xm_lo >> 5;
+    const uint64_t ad = adesc0 + (uint64_t)(s * (TM_A_BYTES >> 4)) + (uint64_t)(kk_lo * 32);
+    const uint64_t bd = bdesc + (uint64_t)(kk_lo * (2 * TM_B_LBO >> 4));
+    tm_wg_fence();
+    tm_wg_fence_regs(acc);
+#pragma unroll
+    for (int k = 0; k < 4; k++) tm_wgmma(acc, ad + (uint64_t)(k * 32), bd + (uint64_t)(k * (2 * TM_B_LBO >> 4)), k > 0);
+    tm_wg_commit();
+    tm_wg_fence_regs(acc);
+}
+static_assert((0 + 63 + 27 + 25) >> 5 <= 3 && (64 + 27 - 25) >> 5 >= 2 && (64 + 63 + 27 + 25) >> 5 <= 5, "4 k-steps per warpgroup cover the widest band");
+
 // ---------------------------------------------------------------------------------------------------
 template <bool PROF>
 __global__ void __launch_bounds__(TM_THREADS, 1) k_threshold_mma(const ThreshMmaArgs a, const __grid_constant__ CUtensorMap tmap) {
@@ -278,14 +306,14 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_threshold_mma(const ThreshMma
     uint8_t* sStage = tm_smem_raw + TM_OFF_STAGE;
     uint32_t* sColw = reinterpret_cast<uint32_t*>(tm_smem_raw + TM_OFF_COLW);
     uint64_t* bar = reinterpret_cast<uint64_t*>(tm_smem_raw + TM_OFF_BAR);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + TMB_COUNT);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, lane = tid & 31;
+    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // provably warp-uniform: the role branches stay convergent for wgmma
     const int total_tiles = a.tiles_x * a.tiles_y * a.n_frames;
 
-    // ---- one-time setup: Hankel band tables, barriers, TMEM ----
+    // ---- one-time setup: Hankel band tables, barriers ----
     for (int w = tid; w < TM_NTAB * TM_A_BYTES / 4; w += TM_THREADS) {
         const int tb = w / (TM_A_BYTES / 4), e = (w - tb * (TM_A_BYTES / 4)) * 4;
-        const int r = tb == 0 ? 0 : 2 * tb - 1;
+        const int r = 2 * tb + 1;
         const int d = e >> 7, row = (e >> 4) & 7, col = e & 15;
         uint32_t v = 0;
 #pragma unroll
@@ -303,27 +331,14 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_threshold_mma(const ThreshMma
         }
         for (int i = 0; i < 2; i++) {
             tm_mbar_init(&bar[TMB_B_FULL + i], TM_NCONV * 32);
-            tm_mbar_init(&bar[TMB_B_EMPTY + i], 1);
+            tm_mbar_init(&bar[TMB_B_EMPTY + i], TM_NEPI);
             tm_mbar_init(&bar[TMB_COLW_FULL + i], TM_NEPI);
             tm_mbar_init(&bar[TMB_COLW_EMPTY + i], TM_NCONV);
         }
-        tm_mbar_init(&bar[TMB_G_FULL], 1);
-        tm_mbar_init(&bar[TMB_G_EMPTY], TM_NEPI);
-        for (int i = 0; i < 4; i++) {
-            tm_mbar_init(&bar[TMB_D_FULL + i], 1);
-            tm_mbar_init(&bar[TMB_D_EMPTY + i], 4);
-        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tm_smem(tmem_slot)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     tm_fence_async_smem();  // the band tables are read by the tensor core (async proxy)
-    tm_fence_before();
     __syncthreads();
-    tm_fence_after();
-    const uint32_t tmem = *tmem_slot;
     long long prof_acc[PROF ? TM_PROF_KINDS : 1];
 #pragma unroll
     for (int i = 0; i < (PROF ? TM_PROF_KINDS : 1); i++) prof_acc[i] = 0;
@@ -352,51 +367,7 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_threshold_mma(const ThreshMma
                 __syncwarp();
             }
         }
-      } else if (warp == TM_WARP_MMA) {
-        // ===== MMA issuer (warp-uniform loop; one elected lane issues the MMAs and the commits) =====
-        // per tile: scales 0 and 1, the centre-pixel product, scales 2..12 -- the first two only need a free accumulator of the
-        // previous tile's scales 9 / 10, so they run under the epilogue of its last scales; g waits for all of them
-        const uint32_t idesc_d = (2u << 4) | ((uint32_t)(TM_N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);   // S32 accum, u8 x u8, K-major both, M 128, N 112
-        const uint32_t idesc_g = (2u << 4) | ((uint32_t)(TM_GN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);  // N 64
-        const uint64_t adesc0 = tm_desc(tm_smem(sA), 256, 128);            // + table * (TM_A_BYTES >> 4) + kstep * 32
-        const uint64_t bdesc0 = tm_desc(tm_smem(sB), TM_B_LBO, 128);       // + buf * (TM_B_BYTES >> 4) + kstep * (2 * TM_B_LBO >> 4) [+ row offset]
-        uint32_t it = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, it++) {
-            const uint32_t buf = it & 1u, useb = it >> 1;
-            TM_WAIT(3, &bar[TMB_B_FULL + buf], useb & 1u);
-            tm_fence_after();
-            const uint64_t bdesc = bdesc0 + (uint64_t)(buf * (TM_B_BYTES >> 4));
-            for (int step = 0; step < TM_NTAB; step++) {
-                const int tb = step < 2 ? step + 1 : (step == 2 ? 0 : step);  // table: 0 = centre pixel, 1 + s = scale s
-                const int r = tb == 0 ? 0 : 2 * tb - 1;
-                uint32_t dcol, idesc;
-                uint64_t bd = bdesc;
-                uint64_t* done;
-                if (tb == 0) {
-                    TM_WAIT(4, &bar[TMB_G_EMPTY], (it & 1u) ^ 1u);
-                    dcol = tmem + TM_GCOL;
-                    idesc = idesc_g;
-                    bd += TM_GROW0;  // B rows 25..88 (16 bytes per row in the row-contiguous layout)
-                    done = &bar[TMB_G_FULL];
-                } else {
-                    const uint32_t j = it * 13u + (uint32_t)(tb - 1), slot = tm_slot_of(j);
-                    TM_WAIT(5, &bar[TMB_D_EMPTY + slot], (tm_slot_use(j) & 1u) ^ 1u);
-                    dcol = tmem + slot * TM_DCOLS;
-                    idesc = idesc_d;
-                    done = &bar[TMB_D_FULL + slot];
-                }
-                tm_fence_after();
-                const int kk_lo = (27 - r) >> 5, kk_hi = (TM_C0 + r) >> 5;  // k-steps that meet the band of any lane
-                const uint64_t ad = adesc0 + (uint64_t)(tb * (TM_A_BYTES >> 4));
-                if (tm_elect()) {
-                    for (int kk = kk_lo; kk <= kk_hi; kk++) tm_mma_i8(dcol, ad + (uint64_t)(kk * 32), bd + (uint64_t)(kk * (2 * TM_B_LBO >> 4)), idesc, kk > kk_lo);
-                    tm_commit(done);
-                    if (step == TM_NTAB - 1) tm_commit(&bar[TMB_B_EMPTY + buf]);  // every MMA that reads this gray tile has completed
-                }
-                __syncwarp();
-            }
-        }
-      }  // warps 2, 3: no role (they complete the first warpgroup so that setmaxnreg can hand its registers to the epilogue)
+      }  // warps 1-3: no role (they complete the first warpgroup so that setmaxnreg can hand its registers to the epilogue)
     } else if (warp < TM_WARP_EPI0) {
         // ===== converters: BGR -> gray into the MMA's B operand; then the halo tiles of the previous tile: the epilogue's
         //       column words (shared memory) -> 32x32 bit transposes -> one 128-byte store per tile and scale =====
@@ -486,14 +457,19 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_threshold_mma(const ThreshMma
             }
         }
     } else {
-        // ===== epilogue: vertical running sums, compare -> column words (shared memory) -> start cracks of the border walk =====
+        // ===== MMA + epilogue: per scale one wgmma chain (64 columns x 112 region rows) into registers, parked in shared
+        //       memory; vertical running sums, compare -> column words (shared memory) -> start cracks of the border walk =====
         tm_regs_inc<TM_REGS_EPI>();
         const int ew = warp - TM_WARP_EPI0;       // 0..7
-        const int G = ew >> 2;                    // scale group: global scale index j with (j & 1) == G
-        const int quarter = warp & 3;             // TMEM lane quarter this warp may read
-        const int mlane = quarter * 32 + lane;    // accumulator row = 127 - xm
-        const int xm = 127 - mlane;               // column index within the tile's 122-column span (x = X0 - 1 + xm)
-        const uint32_t lane_addr = (uint32_t)(quarter * 32) << 16;
+        const int G = ew >> 2;                    // warpgroup: accumulator rows m = 64 G .. 64 G + 63 of the band matrix
+        const int wq = ew & 3;                    // warp inside the warpgroup
+        const int band = wq >> 1;                 // output rows 30 band .. 30 band + 31 (= halo tile row `band` of the tile)
+        const int cl = ((wq & 1) << 5) | lane;    // this thread's column inside the warpgroup's 64
+        const int xm = 127 - (64 * G + cl);       // column index within the tile's 122-column span (x = X0 - 1 + xm)
+        const int y0 = 30 * band;
+        const int xm_lo = G ? 0 : 64;             // columns of the warpgroup: xm_lo .. xm_lo + 63
+        uint16_t* sD = reinterpret_cast<uint16_t*>(tm_smem_raw + TM_OFF_D + 2 * G * TM_D_BYTES);
+        const uint64_t adesc0 = tm_desc(tm_smem(sA) + 1024u * (uint32_t)G, 256, 128);  // + table * (TM_A_BYTES >> 4) + kstep * 32
         const int twoC = 2 * a.thresh_c - 1;
         // this column inside its halo tile: xm = 1..120 are interior columns of tile (xm - 1) / 30 (local column 1..30)
         const int txl = xm >= 1 && xm <= 120 ? (xm - 1) / FID_HALO_T : -1;
@@ -501,6 +477,9 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_threshold_mma(const ThreshMma
         StartAlloc alL{0u, (unsigned int)TM_START_BLOCK}, alR{0u, (unsigned int)TM_START_BLOCK};  // "block used up": the first reservation fetches one
         const unsigned int start_cap = a.max_starts / 2;
         bool start_overflow = false;
+        uint32_t acc[56];
+#pragma unroll
+        for (int i = 0; i < 56; i++) acc[i] = 0;
         uint32_t it = 0;
         for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, it++) {
             int f, bx, by;
@@ -508,143 +487,116 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_threshold_mma(const ThreshMma
             const int X0 = bx * THR_OW, Y0 = by * THR_OH;
             const uint32_t buf = it & 1u, useb = it >> 1;
             uint32_t* colw = sColw + buf * TM_COLW_WORDS;
-            TM_WAIT(8, &bar[TMB_COLW_EMPTY + buf], (useb & 1u) ^ 1u);  // the tail warps are done with this buffer (tile it - 2)
-            // validity: band 0 bit b <-> image row Y0-1+b, band 1 bit b <-> Y0+29+b; column X0-1+xm
-            uint32_t rowmask0 = 0, rowmask1 = 0;
+            TM_WAIT(8, &bar[TMB_COLW_EMPTY + buf], (useb & 1u) ^ 1u);  // the converter warps are done with this buffer (tile it - 2)
+            // validity: bit b of the band's word <-> image row Y0 - 1 + y0 + b; column X0 - 1 + xm
+            uint32_t rowmask;
             {
-                const int lo0 = 1 - Y0, hi0 = a.H - Y0;  // valid b: lo0 <= b <= hi0
-                const int lo1 = -29 - Y0, hi1 = a.H - 30 - Y0;
-                const uint32_t m_lo0 = lo0 <= 0 ? 0xffffffffu : (lo0 >= 32 ? 0u : (0xffffffffu << lo0));
-                const uint32_t m_hi0 = hi0 >= 31 ? 0xffffffffu : (hi0 < 0 ? 0u : (0xffffffffu >> (31 - hi0)));
-                const uint32_t m_lo1 = lo1 <= 0 ? 0xffffffffu : (lo1 >= 32 ? 0u : (0xffffffffu << lo1));
-                const uint32_t m_hi1 = hi1 >= 31 ? 0xffffffffu : (hi1 < 0 ? 0u : (0xffffffffu >> (31 - hi1)));
-                rowmask0 = m_lo0 & m_hi0;
-                rowmask1 = m_lo1 & m_hi1;
+                const int lo = 1 - Y0 - y0, hi = a.H - Y0 - y0;  // valid b: lo <= b <= hi
+                const uint32_t m_lo = lo <= 0 ? 0xffffffffu : (lo >= 32 ? 0u : (0xffffffffu << lo));
+                const uint32_t m_hi = hi >= 31 ? 0xffffffffu : (hi < 0 ? 0u : (0xffffffffu >> (31 - hi)));
+                rowmask = m_lo & m_hi;
             }
             const int X = X0 - 1 + xm;
             const bool col_ok = X >= 0 && X < a.W;
-            bool g_ready = false;
+            TM_WAIT(3, &bar[TMB_B_FULL + buf], useb & 1u);
+            const uint8_t* gB = sB + buf * TM_B_BYTES;
+            // centre pixels of the band's 32 output rows (region rows 25 + y0 ..), region column xm + 27, straight from the gray tile
+            uint32_t g4[8];
+            {
+                const int ic = xm + 27;
+                const uint8_t* gp = gB + (ic >> 4) * TM_B_LBO + (25 + y0) * 16 + (ic & 15);
+#pragma unroll
+                for (int w = 0; w < 8; w++)
+                    g4[w] = (uint32_t)gp[64 * w] | ((uint32_t)gp[64 * w + 16] << 8) | ((uint32_t)gp[64 * w + 32] << 16) | ((uint32_t)gp[64 * w + 48] << 24);
+            }
+            const uint64_t bdesc = tm_desc(tm_smem(gB), TM_B_LBO, 128);  // + kstep * (2 * TM_B_LBO >> 4)
+            tm_issue_scale(acc, adesc0, bdesc, 0, xm_lo);
             for (int s = 0; s < 13; s++) {
-                const uint32_t j = it * 13u + (uint32_t)s;
-                if ((int)(j & 1u) != G) continue;
-                const uint32_t slot = tm_slot_of(j);
-                if (!g_ready) {
-                    TM_WAIT(6, &bar[TMB_G_FULL], it & 1u);
-                    g_ready = true;
+                const uint32_t j = it * 13u + (uint32_t)s;  // global scale index: 13 is odd, so the parking buffers alternate across tiles too
+                uint16_t* sDj = sD + (j & 1u) * (TM_D_BYTES / 2);
+                tm_wg_wait0();
+                tm_wg_fence_regs(acc);
+                {  // park: H(column m, region row n) at sDj[m * TM_DSTRIDE + n], two rows per word
+                    uint32_t* d32 = reinterpret_cast<uint32_t*>(sDj);
+                    const int m0 = 16 * wq + (lane >> 2);
+#pragma unroll
+                    for (int jj = 0; jj < TM_N / 8; jj++)
+#pragma unroll
+                        for (int h = 0; h < 2; h++)
+                            d32[(m0 + 8 * h) * (TM_DSTRIDE / 2) + 4 * jj + (lane & 3)] = (acc[4 * jj + 2 * h] & 0xffffu) | (acc[4 * jj + 2 * h + 1] << 16);
                 }
-                TM_WAIT(7, &bar[TMB_D_FULL + slot], tm_slot_use(j) & 1u);
-                tm_fence_after();
+                if (s == 12) {  // every MMA of this warp that reads the gray tile has completed, and its centre pixels are in registers
+                    __syncwarp();
+                    if (lane == 0) tm_mbar_arrive(&bar[TMB_B_EMPTY + buf]);
+                }
+                asm volatile("bar.sync %0, 128;" ::"r"(2 + G) : "memory");  // the warpgroup's parked scale is complete
+                if (s < 12) tm_issue_scale(acc, adesc0, bdesc, s + 1, xm_lo);  // waited for at once (see the header)
                 const int r = 1 + 2 * s, k = 2 * r + 1, k2 = k * k;
                 const int ck = (twoC * k2 + 1) / 2;  // exact: odd * odd + 1 is even
                 const int negk2 = -k2;
-                const uint32_t dcol = tmem + lane_addr + slot * TM_DCOLS;
-                const uint32_t gcol = tmem + lane_addr + TM_GCOL;  // column = output row (region row - 25)
-                // V = sum of H over rows 25-r .. 25+r of the region (window of output row 0), minus the constant
+                const uint16_t* hc = sDj + cl * TM_DSTRIDE + y0;  // H(x, region row y0 + n)
+                // V = sum of H over region rows y0 + 25 - r .. y0 + 25 + r (window of the band's first output row), minus the constant
                 int V = -ck;
-                {
-                    uint32_t v[16];
-                    int c = 0;
-#pragma unroll 1
-                    for (; c + 16 <= k; c += 16) {  // full chunks: 8 three-input adds
-                        tm_ld16(dcol + (uint32_t)(25 - r + c), v);
-                        tm_ld_wait();
+#pragma unroll 4
+                for (int n = 25 - r; n <= 25 + r; n++) V += (int)hc[n];
+                const uint16_t* lead = hc + 26 + r;
+                const uint16_t* trail = hc + 25 - r;
+                uint32_t w = 0;
 #pragma unroll
-                        for (int jj = 0; jj < 16; jj += 2) V += (int)v[jj] + (int)v[jj + 1];
-                    }
-                    tm_ld16(dcol + (uint32_t)(25 - r + c), v);  // the last k - c (3, 7, 11 or 15) values
-                    tm_ld_wait();
-                    const int rem = k - c;
-#pragma unroll
-                    for (int jj = 0; jj < 15; jj++) V += (jj < rem) ? (int)v[jj] : 0;
+                for (int i = 0; i < 32; i++) {
+                    const int g = (int)((g4[i >> 2] >> (8 * (i & 3))) & 255u);
+                    const int D = g * negk2 + V;  // S - g k^2 - ck: the pixel is set iff D >= 0
+                    w |= (uint32_t)(D >= 0) << i;
+                    if (i < 31) V += (int)lead[i] - (int)trail[i];
                 }
-                // main loop: two 32-row halves x two 16-row chunks, as a LOOP -- the body must stay resident in the per-scheduler
-                // instruction cache (the fully unrolled form made this warp-specialised kernel instruction-fetch bound)
-                uint32_t w0 = 0, w1 = 0;
-#pragma unroll 1
-                for (int half = 0; half < 2; half++) {
-                    uint32_t w = 0;
-#pragma unroll 1
-                    for (int cc = 0; cc < 2; cc++) {
-                        const uint32_t row0 = (uint32_t)(32 * half + 16 * cc);
-                        uint32_t lead[16], trail[16], g16[16];
-                        tm_ld16(dcol + (uint32_t)(26 + r) + row0, lead);
-                        tm_ld16(dcol + (uint32_t)(25 - r) + row0, trail);
-                        tm_ld16(gcol + row0, g16);
-                        tm_ld_wait();
-#pragma unroll
-                        for (int jj = 0; jj < 16; jj++) {
-                            const int D = (int)g16[jj] * negk2 + V;  // S - g k^2 - ck: the pixel is set iff D >= 0
-                            w = __funnelshift_l((uint32_t)D, w, 1);
-                            V = V + (int)lead[jj] - (int)trail[jj];
-                        }
-                    }
-                    if (half == 0)
-                        w0 = w;
-                    else
-                        w1 = w;
-                }
-                tm_fence_before();
-                __syncwarp();
-                if (lane == 0) tm_mbar_arrive(&bar[TMB_D_EMPTY + slot]);
-                // sign bits were shifted in MSB-first: bit (31 - row) = (D < 0)
-                const uint32_t lo = ~__brev(w0), hi = ~__brev(w1);  // bit row = pixel set, rows 0..31 / 32..63
-                const uint32_t b0 = lo & rowmask0, b1 = ((lo >> 30) | (hi << 2)) & rowmask1;
-                const uint32_t cw0 = col_ok ? b0 : 0u, cw1 = col_ok ? b1 : 0u;
-                colw[(s * 2 + 0) * 128 + xm] = cw0;
-                colw[(s * 2 + 1) * 128 + xm] = cw1;
+                const uint32_t cwb = col_ok ? (w & rowmask) : 0u;
+                colw[(s * 2 + band) * 128 + xm] = cwb;
                 {
                     const long long t0_ = PROF ? clock64() : 0;
-                    asm volatile("bar.sync %0, 128;" ::"r"(1 + G) : "memory");  // the group's 128 column words of this scale are in shared memory
+                    asm volatile("bar.sync 1, 256;" ::: "memory");  // all 128 column words of this scale are in shared memory
                     if (PROF) prof_acc[PROF ? 10 : 0] += clock64() - t0_;
                 }
-                // start cracks of this column, exact local prune; neighbour columns from shared memory.  One band per iteration.
-#pragma unroll 1
-                for (int band = 0; band < 2; band++) {
-                    const uint32_t cwb = band ? cw1 : cw0;
-                    uint32_t Lb = 0, Rb = 0;
-                    if (txl >= 0 && cwb) {
-                        const uint32_t* cp = colw + (s * 2 + band) * 128 + xm;
-                        halo_col_starts(xm >= 2 ? cp[-2] : 0u, cp[-1], cwb, cp[1], cp[2], col, &Lb, &Rb);
-                    }
-                    const unsigned int mine = (unsigned int)__popc(Lb) | ((unsigned int)__popc(Rb) << 16);  // both counts in one scan
-                    unsigned int incl = mine;
+                // start cracks of this column, exact local prune; neighbour columns from shared memory
+                uint32_t Lb = 0, Rb = 0;
+                if (txl >= 0 && cwb) {
+                    const uint32_t* cp = colw + (s * 2 + band) * 128 + xm;
+                    halo_col_starts(xm >= 2 ? cp[-2] : 0u, cp[-1], cwb, cp[1], cp[2], col, &Lb, &Rb);
+                }
+                const unsigned int mine = (unsigned int)__popc(Lb) | ((unsigned int)__popc(Rb) << 16);  // both counts in one scan
+                unsigned int incl = mine;
 #pragma unroll
-                    for (int d = 1; d < 32; d <<= 1) {
-                        const unsigned int tv = __shfl_up_sync(0xffffffffu, incl, d);
-                        if (lane >= d) incl += tv;
+                for (int d = 1; d < 32; d <<= 1) {
+                    const unsigned int tv = __shfl_up_sync(0xffffffffu, incl, d);
+                    if (lane >= d) incl += tv;
+                }
+                const unsigned int tot = __shfl_sync(0xffffffffu, incl, 31);
+                if (tot == 0) continue;
+                unsigned int pl = 0, pr = 0;
+                if (tot & 0xffffu) pl = start_reserve(alL, tot & 0xffffu, a.starts, a.counters, a.max_starts, false, lane) + ((incl - mine) & 0xffffu);
+                if (tot >> 16) pr = start_reserve(alR, tot >> 16, a.starts, a.counters, a.max_starts, true, lane) + ((incl - mine) >> 16);
+                if (mine) {
+                    const uint32_t tx = (uint32_t)(bx * THR_TILES_X + txl), ty = (uint32_t)(by * THR_TILES_Y + band);
+                    const uint32_t rec = start_rec_pack((uint32_t)((f * a.halo_tiles_y + (int)ty) * a.halo_tpr + (int)tx), (uint32_t)s, 0u, (uint32_t)col);
+                    while (Lb) {
+                        const int row = __ffs(Lb) - 1;
+                        Lb &= Lb - 1;
+                        if (pl < start_cap)
+                            a.starts[pl].v = rec | ((uint32_t)row << 5);
+                        else
+                            start_overflow = true;
+                        pl++;
                     }
-                    const unsigned int tot = __shfl_sync(0xffffffffu, incl, 31);
-                    if (tot == 0) continue;
-                    unsigned int pl = 0, pr = 0;
-                    if (tot & 0xffffu) pl = start_reserve(alL, tot & 0xffffu, a.starts, a.counters, a.max_starts, false, lane) + ((incl - mine) & 0xffffu);
-                    if (tot >> 16) pr = start_reserve(alR, tot >> 16, a.starts, a.counters, a.max_starts, true, lane) + ((incl - mine) >> 16);
-                    if (mine) {
-                        const uint32_t tx = (uint32_t)(bx * THR_TILES_X + txl), ty = (uint32_t)(by * THR_TILES_Y + band);
-                        const uint32_t rec = start_rec_pack((uint32_t)((f * a.halo_tiles_y + (int)ty) * a.halo_tpr + (int)tx), (uint32_t)s, 0u, (uint32_t)col);
-                        while (Lb) {
-                            const int row = __ffs(Lb) - 1;
-                            Lb &= Lb - 1;
-                            if (pl < start_cap)
-                                a.starts[pl].v = rec | ((uint32_t)row << 5);
-                            else
-                                start_overflow = true;
-                            pl++;
-                        }
-                        while (Rb) {
-                            const int row = __ffs(Rb) - 1;
-                            Rb &= Rb - 1;
-                            if (pr < start_cap)
-                                a.starts[a.max_starts - 1 - pr].v = rec | ((uint32_t)row << 5);
-                            else
-                                start_overflow = true;
-                            pr++;
-                        }
+                    while (Rb) {
+                        const int row = __ffs(Rb) - 1;
+                        Rb &= Rb - 1;
+                        if (pr < start_cap)
+                            a.starts[a.max_starts - 1 - pr].v = rec | ((uint32_t)row << 5);
+                        else
+                            start_overflow = true;
+                        pr++;
                     }
                 }
             }
-            tm_fence_before();
-            __syncwarp();
-            if (lane == 0) tm_mbar_arrive(&bar[TMB_G_EMPTY]);
             __syncwarp();
             if (lane == 0) tm_mbar_arrive(&bar[TMB_COLW_FULL + buf]);  // this warp's column words of the tile are in shared memory
         }
@@ -657,9 +609,6 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_threshold_mma(const ThreshMma
         prof_acc[PROF ? 11 : 0] = clock64() - prof_t0;
         for (int i = 0; i < (PROF ? TM_PROF_KINDS : 1); i++) a.prof[((size_t)blockIdx.x * 16 + warp) * TM_PROF_KINDS + i] = prof_acc[i];
     }
-    tm_fence_before();
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512) : "memory");
 }
 
 }  // namespace fid

@@ -27,9 +27,9 @@ FID_HD void jacobi_eigen(double A[N][N], double w[N], double V[N][N]) {
             for (int j = i + 1; j < N; j++) off += A[i][j] * A[i][j];
         }
         if (off <= 1e-40 * diag || off == 0.0) break;
-        // NOTE: keep the rotation loops rolled.  nvcc 12.9 (-O1..-O3, sm_100a) miscompiles the fully
-        // unrolled N=6 instance (eigenvalues wrong, off-diagonal mass not reduced; host build of the
-        // same source is correct) -- found on B200 via tools/debug_pose.cu.
+        // NOTE: keep the rotation loops rolled.  nvcc 12.9 (-O1..-O3) has miscompiled the fully unrolled
+        // N=6 instance (eigenvalues wrong, off-diagonal mass not reduced; host build of the same source is
+        // correct) -- found with tools/debug_pose.cu.
 #pragma unroll 1
         for (int p = 0; p < N - 1; p++)
 #pragma unroll 1
@@ -325,7 +325,15 @@ FID_HD void homography4(const double src[4][2], const double dst[4][2], double H
 // scaling).  OpenCV uses cv::solve(DECOMP_SVD); for a positive definite system the solutions agree
 // to rounding, so a pivoted elimination is used and the eigen-decomposition (with DECOMP_SVD's
 // singular-value cut-off) is kept only for the rank-deficient case.
-FID_HD void solve_sym6(const double Ain[6][6], const double b[6], double x[6]) {
+// Out of line on the device: inlined into k_pose, nvcc 12.9 (sm_90a, NVVM -O3) miscompiles it -- the LM step comes out
+// wrong and the solver stops after one iteration, rvec off by ~5e-3 (the same source inlined elsewhere, built with
+// -Xcicc -O1, or called out of line gives the host result to 1e-14).
+#if defined(__CUDACC__)
+__host__ __device__ __noinline__
+#else
+inline
+#endif
+void solve_sym6(const double Ain[6][6], const double b[6], double x[6]) {
     double A[6][6];
     for (int i = 0; i < 6; i++) {
         x[i] = b[i];

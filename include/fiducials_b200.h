@@ -1,6 +1,6 @@
 /* fiducials_b200 -- C ABI of libfiducials_b200.so
  *
- * B200-native (sm_100a) replacement for the per-frame hot path of UbiquityRobotics/fiducials:
+ * H100-native (sm_90a) replacement for the per-frame hot path of UbiquityRobotics/fiducials:
  *   aruco_detect  : cv::aruco::detectMarkers + per-marker cv::solvePnP + message arithmetic
  *   fiducial_slam : Map::update (pose fold + map fusion)
  *

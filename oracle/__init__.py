@@ -9,7 +9,7 @@ Parity pinning (see DESIGN.md section "Oracle"):
   * detect/pose: the arithmetic the reference executes at
     aruco_detect/src/aruco_detect.cpp:350 (cv::aruco::detectMarkers), :247
     (cv::solvePnP) and :210 (cv::projectPoints) lives in OpenCV, which is not
-    vendored in /root/reference.  ``aruco_oracle`` drives the OpenCV 4.13 wheel
+    vendored in the reference checkout.  ``aruco_oracle`` drives the OpenCV 4.13 wheel
     of this image (``cv2``) with the reference's parameters
     (aruco_detect.cpp:690-727) and restates the node's own glue arithmetic
     (aruco_detect.cpp:151-221, 447-495).  It is pinned against the reference's

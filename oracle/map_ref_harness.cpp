@@ -1,5 +1,5 @@
 // C interface around the REFERENCE's own Map class (fiducial_slam/src/map.cpp + transform_with_variance.cpp, compiled unmodified
-// from /root/reference against the stand-in headers of oracle/ref_shim -- see oracle/ref_shim/README.md and oracle/Makefile).
+// from the reference checkout against the stand-in headers of oracle/ref_shim -- see oracle/ref_shim/README.md and oracle/Makefile).
 //
 // TEST INFRASTRUCTURE ONLY: the compiled reference is the checker for oracle/slam_oracle.py (tests/test_map_ref.py) and for the CUDA
 // map update (tests/test_gpu_slam.py), and the CPU arm of `bench.py --workload C5`.  Nothing here is linked into the product.

@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device")
 
 
 def _have_gpu():
@@ -46,7 +46,9 @@ def kat():
 
     class Kat:
         def frame(self, name):
-            return cv2.imdecode(z[name + "_png"], cv2.IMREAD_COLOR)
+            """BGR8 pixels, stored losslessly as the top and bottom halves (tests/golden/frames)."""
+            halves = [cv2.imread(os.path.join(ROOT, "tests/golden/frames", "%s_%s.webp" % (name, part)), cv2.IMREAD_COLOR) for part in ("top", "bottom")]
+            return np.ascontiguousarray(np.vstack(halves))
 
         def __getitem__(self, k):
             return z[k]

@@ -411,7 +411,7 @@ def test_full_size_round_trip(det_cache, cfg):
         assert t.image_error < 1.0
 
 
-# ---- the tensor-core threshold kernel (tcgen05.mma kind::i8 + TMEM + TMA; opt-in with FID_THRESH=mma) -------------------
+# ---- the tensor-core threshold kernel (wgmma u8 x u8 -> s32 + TMA; opt-in with FID_THRESH=mma) -------------------
 from fiducials_b200.node import MAXM, Detector, default_params  # noqa: E402
 
 @pytest.fixture

@@ -2,6 +2,7 @@
 (oracle/slam_oracle.py) and the reference's goldens.  Tolerance: map poses within 1e-4 m / 1e-4 rad
 (BASELINE.md section 4); in practice ~1e-12."""
 import math
+import os
 
 import numpy as np
 import pytest
@@ -428,27 +429,52 @@ def test_batch_gauss_newton_refine_matches_oracle():
     slam.close()
 
 
-def test_device_map_matches_the_reference_compiled_code():
-    """The CUDA map update against the REFERENCE'S OWN Map class (oracle/_ref/libmap_ref.so: fiducial_slam/src/map.cpp +
-    transform_with_variance.cpp compiled unmodified against stand-in ROS / tf2 headers; built by oracle/Makefile in the authoring
-    container, shipped prebuilt) -- no restatement in between: per-message robot pose, the full C5 map, links and the map file."""
-    from fiducials_b200 import synth
-    from fiducials_b200.node import FiducialSlam
-    from oracle import map_ref
+MAP_REF_TAPE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "map_ref", "test_device_map_matches_the_reference_compiled_code.npz")
 
-    if not map_ref.available():
-        pytest.skip("oracle/_ref/libmap_ref.so was not built (needs the reference checkout: make -C oracle)")
+
+def _c5_reference_case():
+    from fiducials_b200 import synth
+
     msgs, seed_entry = synth.make_c5_sequence(1000, seed=0)
     text = "%d %.17g %.17g %.17g %.17g %.17g %.17g %.17g 0\n" % tuple(seed_entry[:8])
     T_bc = [0.1, -0.02, 0.3, *so.q_from_rpy(0.02, -0.6, 0.1)]
     inv = so.TWV.from_qt(T_bc[3:], T_bc[:3]).inverse()
     T_cb = [*inv.t, *so.m_to_q(inv.R)]
-    # message by message, with a camera offset: robot pose and variance of every update
+    return msgs, seed_entry, text, T_bc, T_cb
+
+
+def c5_reference_answers():
+    """What the reference's Map returns for the case below: the robot pose of each of the first 120 messages (with a camera
+    offset), the map and links after them, and the map after the whole sequence folded in one replay."""
+    from oracle import map_ref
+
+    msgs, seed_entry, text, T_bc, T_cb = _c5_reference_case()
     ref = map_ref.RefMap(initial_map_text=text)
+    updates = [ref.update(m, T_bc, T_cb) for m in msgs[:120]]
+    entries, links = ref.entries(), ref.links()
+    ref.close()
+    ref = map_ref.RefMap(initial_map_text=text)
+    ref.replay(msgs, [0, 0, 0, 0, 0, 0, 1], [0, 0, 0, 0, 0, 0, 1])
+    entries_all = ref.entries()
+    ref.close()
+    return updates, entries, links, entries_all
+
+
+def test_device_map_matches_the_reference_compiled_code():
+    """The CUDA map update against the REFERENCE'S OWN Map class (oracle/_ref/libmap_ref.so: fiducial_slam/src/map.cpp +
+    transform_with_variance.cpp compiled unmodified against stand-in ROS / tf2 headers by oracle/Makefile, or its answers recorded
+    under tests/golden/map_ref where that library cannot be built) -- no restatement in between: per-message robot pose, the full
+    C5 map and its links."""
+    from fiducials_b200.node import FiducialSlam
+    from oracle import map_ref
+
+    with map_ref.use_tape(MAP_REF_TAPE):
+        updates, re, links, re_all = c5_reference_answers()
+    msgs, seed_entry, text, T_bc, T_cb = _c5_reference_case()
+    # message by message, with a camera offset: robot pose and variance of every update
     slam = FiducialSlam(max_fiducials=512)
     slam.loadMap([seed_entry])
-    for m in msgs[:120]:
-        pub, t, q, cov = ref.update(m, T_bc, T_cb)
+    for m, (pub, t, q, cov) in zip(msgs[:120], updates):
         r = slam.transformCallback(m, np.array(T_bc), np.array(T_cb))
         assert bool(r.valid) == pub
         if pub:
@@ -456,18 +482,12 @@ def test_device_map_matches_the_reference_compiled_code():
             rq = np.array(r.q)
             assert min(np.abs(rq - q).max(), np.abs(rq + q).max()) < 1e-9
             assert abs(r.variance - cov[0]) <= 1e-9 * max(1.0, cov[0])
-    re = ref.entries()
     _cmp_entries(slam.entries(), [(int(x[0]), *x[1:7]) for x in re], 1e-9)
-    assert {k: set(v) for k, v in slam.links().items()} == ref.links()
-    ref.close()
+    assert {k: set(v) for k, v in slam.links().items()} == links
     # the whole sequence in one launch against one replay inside the compiled reference
-    ref = map_ref.RefMap(initial_map_text=text)
-    ref.replay(msgs, [0, 0, 0, 0, 0, 0, 1], [0, 0, 0, 0, 0, 0, 1])
     one = FiducialSlam(max_fiducials=512)
     one.loadMap([seed_entry])
     ident = so.TWV.identity()
     one.replay([msgs], _tf7(ident), _tf7(ident))
-    re = ref.entries()
-    assert len(re) == 500
-    _cmp_entries(one.entries(0), [(int(x[0]), *x[1:7]) for x in re], 1e-8)
-    ref.close()
+    assert len(re_all) == 500
+    _cmp_entries(one.entries(0), [(int(x[0]), *x[1:7]) for x in re_all], 1e-8)

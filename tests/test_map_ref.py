@@ -1,7 +1,9 @@
 """oracle/slam_oracle.py (the numpy restatement every map parity test uses) against the REFERENCE'S OWN Map class: fiducial_slam's
 map.cpp + transform_with_variance.cpp compiled unmodified from the reference checkout against stand-in ROS / tf2 headers
-(oracle/ref_shim, oracle/Makefile -> oracle/_ref/libmap_ref.so).  Same observations in, same map out, to rounding."""
+(oracle/ref_shim, oracle/Makefile -> oracle/_ref/libmap_ref.so), or its answers recorded under tests/golden/map_ref where that
+library cannot be built.  Same observations in, same map out, to rounding."""
 import math
+import os
 
 import numpy as np
 import pytest
@@ -9,7 +11,14 @@ import pytest
 from oracle import map_ref
 from oracle import slam_oracle as so
 
-pytestmark = pytest.mark.skipif(not map_ref.available(), reason="oracle/_ref/libmap_ref.so not built (needs the reference checkout: make -C oracle)")
+TAPES = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "map_ref")
+
+
+@pytest.fixture(autouse=True)
+def reference_answers(request):
+    """The compiled reference where it was built, otherwise its recorded answers for this test (oracle/map_ref.py use_tape)."""
+    with map_ref.use_tape(os.path.join(TAPES, request.node.name + ".npz")):
+        yield
 
 IDENT7 = [0, 0, 0, 0, 0, 0, 1]
 

@@ -1,5 +1,5 @@
 // Debug aid: run solve_marker_pose on host and device from the same translation unit and print the
-// LM trajectory of both.  nvcc -gencode arch=compute_100a,code=sm_100a --fmad=false -DFID_DEBUG_PNP tools/debug_pose.cu
+// LM trajectory of both.  nvcc -gencode arch=compute_90a,code=sm_90a --fmad=false -DFID_DEBUG_PNP tools/debug_pose.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "../fiducials_b200/csrc/pnp.cuh"
