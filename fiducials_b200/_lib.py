@@ -69,6 +69,19 @@ class fid_transform(C.Structure):
     ]
 
 
+class fid_pose_hypotheses(C.Structure):
+    """struct fid_pose_hypotheses: both planar (IPPE_SQUARE) pose solutions of a marker, solvePnPGeneric's order."""
+    _fields_ = [
+        ("fiducial_id", C.c_int32),
+        ("n", C.c_int32),
+        ("iterative_match", C.c_int32),
+        ("reserved", C.c_int32),
+        ("rvec", (C.c_double * 3) * 2),
+        ("tvec", (C.c_double * 3) * 2),
+        ("rms", C.c_double * 2),
+    ]
+
+
 class fid_map_params(C.Structure):
     _fields_ = [
         ("weighting_scale", C.c_double),
@@ -111,7 +124,7 @@ class fid_map_record(C.Structure):
 # every symbol include/fiducials_b200.h declares (tests/test_abi.py checks the list against the header)
 EXPORTS = [
     "fid_strerror", "fid_version", "fid_default_params", "fid_create", "fid_destroy", "fid_set_params", "fid_detect", "fid_pose",
-    "fid_detect_pose_batch", "fid_submit_batch", "fid_collect_batch", "fid_hint_next", "fid_set_input_encoding", "fid_timer_start", "fid_timer_stop", "fid_host_alloc", "fid_host_free", "fid_device_alloc", "fid_device_free", "fid_memcpy_h2d", "fid_debug_threshold", "fid_debug_time_threshold",
+    "fid_detect_pose_batch", "fid_submit_batch", "fid_collect_batch", "fid_set_pose_hypotheses", "fid_pose_hypotheses", "fid_last_pose_hypotheses", "fid_hint_next", "fid_set_input_encoding", "fid_timer_start", "fid_timer_stop", "fid_host_alloc", "fid_host_free", "fid_device_alloc", "fid_device_free", "fid_memcpy_h2d", "fid_debug_threshold", "fid_debug_time_threshold",
     "fid_debug_candidates", "fid_last_stage_ms", "fid_last_counters", "fid_map_default_params", "fid_map_create", "fid_map_destroy", "fid_map_clear",
     "fid_map_load", "fid_map_links", "fid_map_add_links", "fid_map_update", "fid_map_update_sequence", "fid_map_update_frames", "fid_map_update_frames_async", "fid_map_sync", "fid_map_entries", "fid_map_export", "fid_map_merge", "fid_map_export_device",
     "fid_map_merge_device", "fid_map_merge_device_async", "fid_map_export_async", "fid_map_stream", "fid_map_merged_entries", "fid_map_adopt_merged", "fid_map_add_fiducial", "fid_map_refine_default_params", "fid_map_refine",
@@ -142,6 +155,9 @@ def load():
     lib.fid_detect_pose_batch.argtypes = [vp, i32, vp, i32, i32, i32, sz, sz, C.POINTER(fid_camera), C.c_double, i32, vp, vp, i32, vp, vp, vp, vp]
     lib.fid_submit_batch.argtypes = [vp, i32, vp, i32, i32, i32, sz, sz, C.POINTER(fid_camera), C.c_double, i32, vp, vp]
     lib.fid_collect_batch.argtypes = [vp, i32, vp, vp, vp, vp]
+    lib.fid_set_pose_hypotheses.argtypes = [vp, i32]
+    lib.fid_pose_hypotheses.argtypes = [vp, i32, vp, vp, C.POINTER(fid_camera), C.c_double, i32, vp, vp, vp]
+    lib.fid_last_pose_hypotheses.argtypes = [vp, i32, C.POINTER(i32), vp]
     lib.fid_hint_next.argtypes = [vp, vp]
     lib.fid_set_input_encoding.argtypes = [vp, i32]
     lib.fid_debug_time_threshold.argtypes = [vp, i32, vp, i32, i32, sz, sz, i32, C.POINTER(C.c_float)]

@@ -56,11 +56,13 @@ struct Slot {
     int32_t* d_out_ids = nullptr;
     float* d_out_corners = nullptr;
     fid_transform* d_out_tf = nullptr;
+    struct fid_pose_hypotheses* d_out_hyp = nullptr;  // fid_set_pose_hypotheses: allocated by the first enable
     // pinned host mirrors
     int32_t* h_out_count = nullptr;
     int32_t* h_out_ids = nullptr;
     float* h_out_corners = nullptr;
     fid_transform* h_out_tf = nullptr;
+    struct fid_pose_hypotheses* h_out_hyp = nullptr;
     Counters* h_counters = nullptr;
     int* h_nsel = nullptr;
     int* h_nrawc = nullptr;
@@ -90,7 +92,7 @@ struct fid_detector {
     struct Pending {
         int first_slot, n_chunks, n_frames, w, h;
         int64_t launches;
-        bool pose;
+        bool pose, hyp;
     } pending[MAX_SLOTS]{};
     int pend_head = 0, pend_count = 0, slots_in_use = 0, slot_next = 0;
     cudaStream_t slot_stream[MAX_SLOTS] = {};
@@ -118,6 +120,13 @@ struct fid_detector {
     int32_t* d_pose_ids = nullptr;
     float* d_pose_corners = nullptr;
     fid_transform* d_pose_out = nullptr;
+    // both planar pose hypotheses (fid_set_pose_hypotheses / fid_pose_hypotheses / fid_last_pose_hypotheses)
+    int pose_hyp = 0;                                // the batch option
+    struct fid_pose_hypotheses* d_hyp_list = nullptr;  // fid_pose_hypotheses output, 4096 records, allocated by the first call
+    bool last_hyp_valid = false;                     // the batch last returned had the option on (and a camera)
+    int last_hyp_frames = 0, last_hyp_stride = 0;
+    std::vector<int32_t> last_hyp_counts;
+    std::vector<struct fid_pose_hypotheses> last_hyp;  // [last_hyp_frames][last_hyp_stride]
     float stage_ms[ST_COUNT + N_WALK_ROUNDS]{};
     int64_t counters[8]{};
     cudaEvent_t t0 = nullptr, t1 = nullptr;
@@ -302,10 +311,10 @@ static void free_slot(Slot& s) {
                      s.d_raw,         s.d_nraw,          s.fs.quads_tmp,    s.fs.per_tmp,     s.fs.quads,       s.fs.per,         s.fs.close_bits, s.fs.group_id,
                      s.fs.group_members, s.fs.next_in_group, s.fs.group_head, s.fs.group_tail, s.fs.close_count, s.fs.close_idx,   s.fs.close_off,  s.fs.selected,
                      s.fs.sel_idx,    s.d_nsel,          s.d_nrawc,         s.d_cand_id,      s.d_cand_corners, s.d_out_count,    s.d_out_ids,     s.d_out_corners,
-                     s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list};
+                     s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp};
     for (void* p : dptrs)
         if (p) cudaFree(p);
-    void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc};
+    void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp};
     for (void* p : hptrs)
         if (p) cudaFreeHost(p);
     for (int i = 0; i <= ST_COUNT; i++)
@@ -455,7 +464,7 @@ extern "C" int fid_destroy(fid_detector* h) {
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();
     for (int i = 0; i < MAX_SLOTS; i++) free_slot(h->slot[i]);
-    void* ptrs[] = {h->d_prune, h->d_dict, h->d_pf[0], h->d_pf[1], h->d_lut_prev, h->d_lut_next, h->d_subpix_masks, h->d_override_ids, h->d_override_lens, h->d_pose_ids, h->d_pose_corners, h->d_pose_out};
+    void* ptrs[] = {h->d_prune, h->d_dict, h->d_pf[0], h->d_pf[1], h->d_lut_prev, h->d_lut_next, h->d_subpix_masks, h->d_override_ids, h->d_override_lens, h->d_pose_ids, h->d_pose_corners, h->d_pose_out, h->d_hyp_list};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     for (int i = 0; i < 2; i++)
@@ -804,18 +813,35 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         launch_prio(k_finish, dim3(nf), dim3(FINISH_THREADS), 0, st, 5, a);
         launches++;
     }
+    if (h->pose_hyp && cam) {  // opt-in: both planar hypotheses of every marker k_finish wrote (fid_set_pose_hypotheses)
+        PoseHypArgs a{};
+        a.nf = nf;
+        a.max_markers = h->max_markers;
+        a.count = s.d_out_count;
+        a.corners = s.d_out_corners;
+        a.tf = s.d_out_tf;
+        a.cam = make_camera(cam);
+        a.fiducial_len = fiducial_len;
+        a.n_override = n_override;
+        a.override_ids = h->d_override_ids;
+        a.override_lens = h->d_override_lens;
+        a.out = s.d_out_hyp;
+        launch_prio(k_pose_hypotheses, dim3(nf), dim3(POSE_HYP_THREADS), 0, st, 5, a);
+        launches++;
+    }
     CK(cudaEventRecord(s.ev[ST_D2H], st));
     h->counters[6] += launches;
     CK(cudaGetLastError());
     return FID_OK;
 }
 
-static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose) {
+static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose, bool with_hyp) {
     const size_t M = (size_t)nf * h->max_markers;
     CK(cudaMemcpyAsync(s.h_out_count, s.d_out_count, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_out_ids, s.d_out_ids, sizeof(int32_t) * M, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_out_corners, s.d_out_corners, sizeof(float) * 8 * M, cudaMemcpyDeviceToHost, st));
     if (with_pose) CK(cudaMemcpyAsync(s.h_out_tf, s.d_out_tf, sizeof(fid_transform) * M, cudaMemcpyDeviceToHost, st));
+    if (with_hyp) CK(cudaMemcpyAsync(s.h_out_hyp, s.d_out_hyp, sizeof(struct fid_pose_hypotheses) * M, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_counters, s.d_counters, sizeof(Counters), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_nsel, s.d_nsel, sizeof(int) * nf, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_nrawc, s.d_nrawc, sizeof(int) * nf, cudaMemcpyDeviceToHost, st));
@@ -824,7 +850,8 @@ static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool w
     return FID_OK;
 }
 
-static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* tfs, bool first_chunk) {
+static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* tfs, bool first_chunk,
+                   struct fid_pose_hypotheses* hyps = nullptr) {
     CK(cudaEventSynchronize(s.done));
     int status = FID_OK;
     if (s.h_counters->overflow) status = FID_ERR_CAPACITY;
@@ -838,6 +865,7 @@ static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* c
         if (ids) memcpy(ids + (size_t)f * max_markers, s.h_out_ids + (size_t)f * h->max_markers, sizeof(int32_t) * n);
         if (corners) memcpy(corners + (size_t)f * max_markers * 8, s.h_out_corners + (size_t)f * h->max_markers * 8, sizeof(float) * 8 * n);
         if (tfs) memcpy(tfs + (size_t)f * max_markers, s.h_out_tf + (size_t)f * h->max_markers, sizeof(fid_transform) * n);
+        if (hyps) memcpy(hyps + (size_t)f * max_markers, s.h_out_hyp + (size_t)f * h->max_markers, sizeof(struct fid_pose_hypotheses) * n);
     }
     // statistics
     float ms = 0;
@@ -881,6 +909,22 @@ static int upload_overrides(fid_detector* h, int n_override, const int32_t* ids,
     return FID_OK;
 }
 
+// The host copy of the records of the batch being returned (fid_last_pose_hypotheses), dense at the caller's max_markers; nullptr
+// when the option is off for the batch.
+static struct fid_pose_hypotheses* begin_last_hypotheses(fid_detector* h, bool hyp, int n_frames, int max_markers) {
+    h->last_hyp_valid = false;
+    if (!hyp) return nullptr;
+    h->last_hyp_frames = n_frames;
+    h->last_hyp_stride = max_markers;
+    h->last_hyp.resize((size_t)n_frames * max_markers);
+    return h->last_hyp.data();
+}
+static void end_last_hypotheses(fid_detector* h, bool hyp, const int32_t* counts) {
+    if (!hyp) return;
+    h->last_hyp_counts.assign(counts, counts + h->last_hyp_frames);
+    h->last_hyp_valid = true;
+}
+
 extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
                                      const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
                                      int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms) {
@@ -896,6 +940,8 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
     int status = FID_OK;
     const int B = h->max_batch;
     const int n_chunks = (n_frames + B - 1) / B;
+    const bool hyp = h->pose_hyp && cam;
+    struct fid_pose_hypotheses* hyps = begin_last_hypotheses(h, hyp, n_frames, max_markers);
     h->counters[6] = 0;
     h->stage_ms[ST_H2D] = 0;
     // software pipeline over chunks: up to n_slots chunks in flight, each on its own stream; results of
@@ -948,7 +994,7 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
             }
             rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, c > 0 ? &h->slot[(c - 1) % NS] : nullptr);
             if (rc != FID_OK) return rc;
-            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr);
+            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp);
             if (rc != FID_OK) return rc;
             h->last_frames = nf;
         }
@@ -957,10 +1003,12 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
             Slot& s = h->slot[pc % NS];
             const int nf = std::min(B, n_frames - pc * B);
             rc = collect(h, s, nf, max_markers, counts + (size_t)pc * B, ids ? ids + (size_t)pc * B * max_markers : nullptr,
-                         corners ? corners + (size_t)pc * B * max_markers * 8 : nullptr, (transforms && cam) ? transforms + (size_t)pc * B * max_markers : nullptr, pc == 0);
+                         corners ? corners + (size_t)pc * B * max_markers * 8 : nullptr, (transforms && cam) ? transforms + (size_t)pc * B * max_markers : nullptr, pc == 0,
+                         hyps ? hyps + (size_t)pc * B * max_markers : nullptr);
             if (rc != FID_OK) status = rc;
         }
     }
+    end_last_hypotheses(h, hyp, counts);
     return status;
 }
 
@@ -1009,7 +1057,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
         const Slot* prev = (h->slots_in_use + c) > 0 ? &h->slot[(si + NS - 1) % NS] : nullptr;
         rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, prev);
         if (rc != FID_OK) return rc;
-        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr);
+        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam);
         if (rc != FID_OK) return rc;
         h->last_frames = nf;
     }
@@ -1020,6 +1068,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
     pb.w = width;
     pb.h = height;
     pb.pose = cam != nullptr;
+    pb.hyp = h->pose_hyp && cam;
     pb.launches = h->counters[6];
     h->pend_count++;
     h->slots_in_use += n_chunks;
@@ -1035,13 +1084,16 @@ extern "C" int fid_collect_batch(fid_detector* h, int max_markers, int32_t* coun
     int status = FID_OK;
     h->counters[6] = pb.launches;
     h->stage_ms[ST_H2D] = 0;
+    struct fid_pose_hypotheses* hyps = begin_last_hypotheses(h, pb.hyp, pb.n_frames, max_markers);
     for (int c = 0; c < pb.n_chunks; c++) {
         Slot& s = h->slot[(pb.first_slot + c) % NS];
         const int nf = std::min(B, pb.n_frames - c * B);
         const int rc = collect(h, s, nf, max_markers, counts + (size_t)c * B, ids ? ids + (size_t)c * B * max_markers : nullptr,
-                               corners ? corners + (size_t)c * B * max_markers * 8 : nullptr, (transforms && pb.pose) ? transforms + (size_t)c * B * max_markers : nullptr, c == 0);
+                               corners ? corners + (size_t)c * B * max_markers * 8 : nullptr, (transforms && pb.pose) ? transforms + (size_t)c * B * max_markers : nullptr, c == 0,
+                               hyps ? hyps + (size_t)c * B * max_markers : nullptr);
         if (rc != FID_OK) status = rc;
     }
+    end_last_hypotheses(h, pb.hyp, counts);
     h->pend_head = (h->pend_head + 1) % MAX_SLOTS;
     h->pend_count--;
     h->slots_in_use -= pb.n_chunks;
@@ -1080,6 +1132,62 @@ extern "C" int fid_pose(fid_detector* h, int n, const int32_t* ids, const float*
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(out, h->d_pose_out, sizeof(fid_transform) * n, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
+    return FID_OK;
+}
+
+extern "C" int fid_set_pose_hypotheses(fid_detector* h, int enable) {
+    if (!h || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight were enqueued with the old setting
+    if (enable) {  // (a failed allocation leaves the option off; the next enable completes it)
+        CK(cudaSetDevice(h->device));
+        const size_t M = (size_t)h->max_batch * h->max_markers;
+        for (int i = 0; i < h->n_slots; i++) {
+            Slot& s = h->slot[i];
+            int rc;
+            if (!s.d_out_hyp && (rc = dalloc(&s.d_out_hyp, M)) != FID_OK) return rc;
+            if (!s.h_out_hyp && (rc = halloc(&s.h_out_hyp, M)) != FID_OK) return rc;
+        }
+    }
+    h->pose_hyp = enable ? 1 : 0;
+    return FID_OK;
+}
+
+extern "C" int fid_pose_hypotheses(fid_detector* h, int n, const int32_t* ids, const float* corners, const fid_camera* cam, double fiducial_len, int n_override,
+                                   const int32_t* override_ids, const double* override_lens, struct fid_pose_hypotheses* out) {
+    if (!h || n < 0 || n > 4096 || !cam || !(fiducial_len > 0) || (n > 0 && (!ids || !corners || !out))) return FID_ERR_INVALID_ARG;
+    if (h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight read the shared override table
+    if (n == 0) return FID_OK;
+    CK(cudaSetDevice(h->device));
+    int rc = upload_overrides(h, n_override, override_ids, override_lens);
+    if (rc != FID_OK) return rc;
+    if (!h->d_hyp_list && (rc = dalloc(&h->d_hyp_list, 4096)) != FID_OK) return rc;
+    CK(cudaMemcpyAsync(h->d_pose_ids, ids, sizeof(int32_t) * n, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_pose_corners, corners, sizeof(float) * 8 * n, cudaMemcpyHostToDevice, h->stream));
+    PoseHypListArgs a{};
+    a.n = n;
+    a.ids = h->d_pose_ids;
+    a.corners = h->d_pose_corners;
+    a.cam = make_camera(cam);
+    a.fiducial_len = fiducial_len;
+    a.n_override = n_override;
+    a.override_ids = h->d_override_ids;
+    a.override_lens = h->d_override_lens;
+    a.out = h->d_hyp_list;
+    k_pose_hypotheses_list<<<(n + 63) / 64, 64, 0, h->stream>>>(a);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, h->d_hyp_list, sizeof(struct fid_pose_hypotheses) * n, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return FID_OK;
+}
+
+extern "C" int fid_last_pose_hypotheses(fid_detector* h, int max_markers, int* n_frames, struct fid_pose_hypotheses* out) {
+    if (!h || !n_frames || max_markers < 0 || !h->last_hyp_valid) return FID_ERR_INVALID_ARG;
+    const int nf = h->last_hyp_frames;
+    *n_frames = nf;
+    if (!out) return FID_OK;
+    for (int f = 0; f < nf; f++)
+        if (h->last_hyp_counts[f] > max_markers) return FID_ERR_CAPACITY;
+    for (int f = 0; f < nf; f++)
+        memcpy(out + (size_t)f * max_markers, h->last_hyp.data() + (size_t)f * h->last_hyp_stride, sizeof(struct fid_pose_hypotheses) * h->last_hyp_counts[f]);
     return FID_OK;
 }
 

@@ -5,6 +5,7 @@
 //                 check, first-match dictionary search (+ close-contour retry)           (A.6, A.7)
 //   k_finish      one block per frame: compaction in OpenCV's output order, cornerSubPix (A.8),
 //                 solvePnP(ITERATIVE) + FiducialTransform arithmetic                     (A.9)
+//   k_pose_hypotheses  opt-in, after k_finish: both IPPE_SQUARE solutions per marker (ippe.cuh)
 #pragma once
 #include <cuda_runtime.h>
 
@@ -12,6 +13,7 @@
 #include "common.cuh"
 #include "contour_refine.cuh"
 #include "identify.cuh"
+#include "ippe.cuh"
 #include "pnp.cuh"
 #include "quad_group.cuh"
 #include "subpix.cuh"
@@ -746,6 +748,87 @@ __global__ void __launch_bounds__(64) k_pose(const PoseArgs a) {
     t.object_error = po.object_error;
     t.fiducial_area = po.area;
     a.out[m] = t;
+}
+
+
+// ---------------------------------------------------------------------------------------------------
+// Both planar pose hypotheses (ippe.cuh), an opt-in stage of its own so that k_finish and the default pipeline stay as they are.
+__device__ __forceinline__ void pack_hypotheses(int id, const PoseHypOut& ho, struct fid_pose_hypotheses* r) {
+    struct fid_pose_hypotheses t;
+    t.fiducial_id = id;
+    t.n = ho.n;
+    t.iterative_match = ho.iterative_match;
+    t.reserved = 0;
+    for (int s = 0; s < 2; s++) {
+        for (int k = 0; k < 3; k++) {
+            t.rvec[s][k] = ho.rvec[s][k];
+            t.tvec[s][k] = ho.tvec[s][k];
+        }
+        t.rms[s] = ho.rms[s];
+    }
+    *r = t;
+}
+
+__device__ __forceinline__ double marker_len_of(int id, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens) {
+    double len = (double)(float)fiducial_len;  // as k_finish / k_pose
+    for (int k = 0; k < n_override; k++)
+        if (override_ids[k] == id) len = override_lens[k];
+    return len;
+}
+
+struct PoseHypArgs {
+    int nf, max_markers;
+    const int32_t* count;         // [F]                   k_finish's outputs
+    const float* corners;         // [F][max_markers][8]
+    const fid_transform* tf;      // [F][max_markers]      the ITERATIVE pose (rvec) and the id
+    Camera cam;
+    double fiducial_len;
+    int n_override;
+    const int32_t* override_ids;
+    const double* override_lens;
+    struct fid_pose_hypotheses* out;  // [F][max_markers]; slots past count[f] are not written
+};
+
+#define POSE_HYP_THREADS 32
+
+// One block per frame, one thread per marker.
+__global__ void __launch_bounds__(POSE_HYP_THREADS) k_pose_hypotheses(const PoseHypArgs a) {
+    const int f = blockIdx.x;
+    const int n = a.count[f];
+    for (int m = threadIdx.x; m < n; m += POSE_HYP_THREADS) {
+        const size_t o = (size_t)f * a.max_markers + m;
+        const fid_transform& t = a.tf[o];
+        const int id = t.fiducial_id;
+        const double rit[3] = {t.rvec[0], t.rvec[1], t.rvec[2]};
+        PoseHypOut ho;
+        solve_marker_hypotheses(a.corners + o * 8, a.cam, (float)marker_len_of(id, a.fiducial_len, a.n_override, a.override_ids, a.override_lens), rit, &ho);
+        pack_hypotheses(id, ho, a.out + o);
+    }
+}
+
+// Host corners (fid_pose_hypotheses): one thread per marker of a single list; the ITERATIVE pose is solved here as k_pose does.
+struct PoseHypListArgs {
+    int n;
+    const int32_t* ids;
+    const float* corners;
+    Camera cam;
+    double fiducial_len;
+    int n_override;
+    const int32_t* override_ids;
+    const double* override_lens;
+    struct fid_pose_hypotheses* out;
+};
+
+__global__ void __launch_bounds__(64) k_pose_hypotheses_list(const PoseHypListArgs a) {
+    const int m = blockIdx.x * blockDim.x + threadIdx.x;
+    if (m >= a.n) return;
+    const int id = a.ids[m];
+    const float len = (float)marker_len_of(id, a.fiducial_len, a.n_override, a.override_ids, a.override_lens);
+    PoseOut po;
+    solve_marker_pose(a.corners + (size_t)m * 8, a.cam, len, a.fiducial_len, &po);
+    PoseHypOut ho;
+    solve_marker_hypotheses(a.corners + (size_t)m * 8, a.cam, len, po.rvec, &ho);
+    pack_hypotheses(id, ho, a.out + m);
 }
 
 }  // namespace fid

@@ -155,6 +155,31 @@ class Detector:
                                               C.cast(tfs, C.c_void_p) if tfs is not None else None), "fid_collect_batch")
         return counts, ids, corners, tfs
 
+    def set_pose_hypotheses(self, enable: bool):
+        """fid_set_pose_hypotheses: batches submitted from now on also compute both planar pose solutions of every marker."""
+        _lib.check(self.lib.fid_set_pose_hypotheses(self.h, int(bool(enable))), "fid_set_pose_hypotheses")
+
+    def pose_hypotheses(self, ids, corners, K, D, fiducial_len, overrides: Optional[Dict[int, float]] = None):
+        """fid_pose_hypotheses: both IPPE_SQUARE solutions of markers already detected (arguments as pose())."""
+        ids = np.ascontiguousarray(ids, np.int32)
+        corners = np.ascontiguousarray(corners, np.float32).reshape(-1, 8)
+        n = len(ids)
+        out = (_lib.fid_pose_hypotheses * max(n, 1))()
+        cam = _camera(K, D)
+        oi, ol, no = _overrides(overrides)
+        _lib.check(self.lib.fid_pose_hypotheses(self.h, n, ids.ctypes.data_as(C.c_void_p), corners.ctypes.data_as(C.c_void_p), C.byref(cam), float(fiducial_len), no,
+                                                oi.ctypes.data_as(C.c_void_p), ol.ctypes.data_as(C.c_void_p), C.cast(out, C.c_void_p)), "fid_pose_hypotheses")
+        return [out[i] for i in range(n)]
+
+    def last_pose_hypotheses(self, max_markers=MAXM):
+        """fid_last_pose_hypotheses: records of the batch last returned by detect_pose_batch / collect_batch, as a ctypes array
+        [n_frames * max_markers] laid out like its transforms (record f * max_markers + m belongs to marker m of frame f)."""
+        nf = C.c_int(0)
+        _lib.check(self.lib.fid_last_pose_hypotheses(self.h, max_markers, C.byref(nf), None), "fid_last_pose_hypotheses")
+        out = (_lib.fid_pose_hypotheses * max(nf.value * max_markers, 1))()
+        _lib.check(self.lib.fid_last_pose_hypotheses(self.h, max_markers, C.byref(nf), C.cast(out, C.c_void_p)), "fid_last_pose_hypotheses")
+        return out
+
     def debug_threshold(self, bgr):
         bgr = np.ascontiguousarray(bgr, np.uint8)
         H, W = bgr.shape[:2]
@@ -203,7 +228,8 @@ class FiducialsNode:
     """aruco_detect's node, minus ROS transport."""
 
     def __init__(self, dictionary=7, fiducial_len=0.14, ignore_fiducials: Iterable[int] = (), fiducial_len_override: Optional[Dict[int, float]] = None,
-                 do_pose_estimation=True, device=0, max_width=1920, max_height=1080, max_batch=1, doCornerRefinement=True, cornerRefinementSubPix=True, **detector_params):
+                 do_pose_estimation=True, device=0, max_width=1920, max_height=1080, max_batch=1, doCornerRefinement=True, cornerRefinementSubPix=True, pose_hypotheses=False,
+                 **detector_params):
         # doCornerRefinement / cornerRefinementSubPix -> cornerRefinementMethod NONE / SUBPIX / CONTOUR (:700-711, configCallback :274-281)
         detector_params.setdefault("cornerRefinementMethod", (1 if cornerRefinementSubPix else 2) if doCornerRefinement else 0)
         self.fiducial_len = float(fiducial_len)  # :615
@@ -211,6 +237,11 @@ class FiducialsNode:
         self.ignoreIds = set(int(i) for i in ignore_fiducials)  # :540-571
         self.fiducialLens = dict(fiducial_len_override or {})  # :627-660
         self.det = Detector(default_params(dictionary=dictionary, **detector_params), device, max_width, max_height, max_batch)
+        # both planar pose solutions of every marker (new, no reference counterpart): when on, the pose results carry an extra
+        # attribute `pose_hypotheses` = {fiducial_id: fid_pose_hypotheses record}; their message fields are unchanged
+        self.poseHypotheses = bool(pose_hypotheses)
+        if self.poseHypotheses:
+            self.det.set_pose_hypotheses(True)
         self.haveCamInfo = False
         self.K = None
         self.D = None
@@ -263,6 +294,7 @@ class FiducialsNode:
             return None  # :417-422
         try:
             tfs = self.det.pose(self.ids, self.corners, self.K, self.D, self.fiducial_len, self.fiducialLens)
+            hyps = self.det.pose_hypotheses(self.ids, self.corners, self.K, self.D, self.fiducial_len, self.fiducialLens) if self.poseHypotheses else None
         except _lib.FidError:
             return fta
         if self.vis_msgs:  # :403, :462-478: vision_msgs/Detection2DArray instead of FiducialTransformArray
@@ -271,18 +303,26 @@ class FiducialsNode:
                 if t.fiducial_id in self.ignoreIds:
                     continue
                 vma.detections.append(Detection2D([ObjectHypothesisWithPose(int(t.fiducial_id), math.exp(-2.0 * float(t.object_error)), tuple(t.translation), tuple(t.rotation))]))
+            if hyps is not None:
+                vma.pose_hypotheses = self._by_id(hyps)
             return vma
         for t in tfs:
             if t.fiducial_id in self.ignoreIds:
                 continue  # :440
             fta.transforms.append(_to_msg(t))
+        if hyps is not None:
+            fta.pose_hypotheses = self._by_id(hyps)
         return fta
+
+    def _by_id(self, records):
+        return {int(r.fiducial_id): r for r in records if r.fiducial_id not in self.ignoreIds}
 
     def process_batch(self, frames, first_seq=0) -> List[FiducialTransformArray]:
         """Throughput path: detect + pose for a stack of frames in one C-ABI call."""
         if not self.haveCamInfo:
             return []
         counts, ids, corners, tfs = self.det.detect_pose_batch(frames, self.K, self.D, self.fiducial_len, self.fiducialLens)
+        hyps = self.det.last_pose_hypotheses() if self.poseHypotheses else None
         out = []
         for f in range(len(counts)):
             fta = FiducialTransformArray(header=Header(0, (0, 0), self.frameId), image_seq=first_seq + f)
@@ -290,6 +330,8 @@ class FiducialsNode:
                 t = tfs[f * MAXM + m]
                 if t.fiducial_id not in self.ignoreIds:
                     fta.transforms.append(_to_msg(t))
+            if hyps is not None:
+                fta.pose_hypotheses = self._by_id(hyps[f * MAXM + m] for m in range(int(counts[f])))
             out.append(fta)
         return out
 

@@ -140,6 +140,40 @@ int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_
                      const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens);
 int fid_collect_batch(fid_detector* h, int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms);
 
+/* Both planar pose solutions of a marker (NEW; the reference publishes only the cv::solvePnP(SOLVEPNP_ITERATIVE) pose of
+ * aruco_detect.cpp:247, and so does fid_transform).  A square seen small, far away or nearly fronto-parallel fits two poses
+ * almost equally well, and ITERATIVE may settle in either.  Each record restates cv::solvePnPGeneric(obj, corners, K, D, rvecs,
+ * tvecs, false, SOLVEPNP_IPPE_SQUARE, noArray(), noArray(), rms) of OpenCV 4.13 (IPPE::PoseSolver::solveSquare) on the object
+ * points of estimatePoseSingleMarkers (getSingleMarkerObjectPoints :151-161, fiducial_len and its overrides narrowed to float):
+ * the two solutions in solvePnPGeneric's order (by the IPPE solver's own error in normalised coordinates), each with the
+ * reprojection RMS solvePnPGeneric reports (projectPoints with K and D, norm / sqrt(2n), px).  iterative_match = index of the
+ * solution whose rotation is closer to the ITERATIVE pose of the marker's fid_transform: 0 when the published pose is the
+ * better-fitting hypothesis, 1 when it is the other one.  n = 0 (everything else 0, iterative_match -1) where solvePnPGeneric
+ * finds no solution: a degenerate quad.  The published pose and every other output are unchanged.
+ * A struct tag without a typedef: the plain name is the function fid_pose_hypotheses below, so write `struct fid_pose_hypotheses`. */
+struct fid_pose_hypotheses {
+    int32_t fiducial_id;
+    int32_t n;                /* 2; 0 if IPPE found no solution (degenerate quad) */
+    int32_t iterative_match;  /* which of the two the ITERATIVE pose of fid_transform lies in; -1 when n == 0 */
+    int32_t reserved;
+    double rvec[2][3], tvec[2][3];
+    double rms[2];            /* reprojection RMS in px, in cv::solvePnPGeneric's order */
+};
+
+/* Opt-in second pose stage of the batch calls (default off): with it on, every batch submitted with a camera also computes the
+ * records of its markers on the device, after the ITERATIVE pose, and copies them back with the other results.  Not while
+ * batches are in flight (like fid_set_input_encoding).  The first enable allocates the result buffers. */
+int fid_set_pose_hypotheses(fid_detector* h, int enable);
+/* Records for markers already detected, the counterpart of fid_pose (same arguments, same object points and overrides); it runs
+ * the ITERATIVE solve of fid_pose itself for iterative_match.  Works whether or not the batch option is on. */
+int fid_pose_hypotheses(fid_detector* h, int n, const int32_t* ids, const float* corners, const fid_camera* cam, double fiducial_len, int n_override,
+                        const int32_t* override_ids, const double* override_lens, struct fid_pose_hypotheses* out);
+/* Records of the batch most recently returned by fid_collect_batch / fid_detect_pose_batch, dense [n_frames][max_markers] in
+ * the marker order of that batch's ids and transforms (records past counts[f] are not written).  *n_frames = the batch's frame
+ * count; out may be NULL to query it.  FID_ERR_INVALID_ARG if the option was off for that batch (or it had no camera);
+ * FID_ERR_CAPACITY, with nothing written, if a frame of the batch has more markers than max_markers. */
+int fid_last_pose_hypotheses(fid_detector* h, int max_markers, int* n_frames, struct fid_pose_hypotheses* out);
+
 /* Pixel format of the frames handed to every entry point that takes `bgr` (default FID_ENC_BGR8).  The
  * reference converts whatever the camera publishes with cv_bridge::toCvCopy(msg, BGR8)
  * (aruco_detect.cpp:348) before detectMarkers turns it into gray again; the library takes the camera's own
