@@ -7,6 +7,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <vector>
 
 #include "../../include/fiducials_b200.h"
@@ -57,12 +58,14 @@ struct Slot {
     float* d_out_corners = nullptr;
     fid_transform* d_out_tf = nullptr;
     struct fid_pose_hypotheses* d_out_hyp = nullptr;  // fid_set_pose_hypotheses: allocated by the first enable
+    fid_board_pose* d_out_board = nullptr;             // fid_set_boards: [max_batch][FID_MAX_BOARDS], allocated by the first set
     // pinned host mirrors
     int32_t* h_out_count = nullptr;
     int32_t* h_out_ids = nullptr;
     float* h_out_corners = nullptr;
     fid_transform* h_out_tf = nullptr;
     struct fid_pose_hypotheses* h_out_hyp = nullptr;
+    fid_board_pose* h_out_board = nullptr;
     Counters* h_counters = nullptr;
     int* h_nsel = nullptr;
     int* h_nrawc = nullptr;
@@ -92,7 +95,7 @@ struct fid_detector {
     struct Pending {
         int first_slot, n_chunks, n_frames, w, h;
         int64_t launches;
-        bool pose, hyp;
+        bool pose, hyp, board;
     } pending[MAX_SLOTS]{};
     int pend_head = 0, pend_count = 0, slots_in_use = 0, slot_next = 0;
     cudaStream_t slot_stream[MAX_SLOTS] = {};
@@ -127,6 +130,15 @@ struct fid_detector {
     int last_hyp_frames = 0, last_hyp_stride = 0;
     std::vector<int32_t> last_hyp_counts;
     std::vector<struct fid_pose_hypotheses> last_hyp;  // [last_hyp_frames][last_hyp_stride]
+    // one pose per board (fid_set_boards / fid_estimate_board_poses / fid_last_board_poses)
+    int n_boards = 0;                                // 0 = off
+    int32_t *d_board_off = nullptr, *d_board_keys = nullptr, *d_board_marker = nullptr;  // see BoardPoseArgs
+    float* d_board_obj = nullptr;
+    int32_t* d_board_count = nullptr;                // fid_estimate_board_poses: the list's length
+    fid_board_pose* d_board_list = nullptr;          // fid_estimate_board_poses output, FID_MAX_BOARDS records
+    bool last_board_valid = false;                   // the batch last returned had boards (and a camera)
+    int last_board_frames = 0, last_board_n = 0;
+    std::vector<fid_board_pose> last_board;          // [last_board_frames][last_board_n]
     float stage_ms[ST_COUNT + N_WALK_ROUNDS]{};
     int64_t counters[8]{};
     cudaEvent_t t0 = nullptr, t1 = nullptr;
@@ -311,10 +323,10 @@ static void free_slot(Slot& s) {
                      s.d_raw,         s.d_nraw,          s.fs.quads_tmp,    s.fs.per_tmp,     s.fs.quads,       s.fs.per,         s.fs.close_bits, s.fs.group_id,
                      s.fs.group_members, s.fs.next_in_group, s.fs.group_head, s.fs.group_tail, s.fs.close_count, s.fs.close_idx,   s.fs.close_off,  s.fs.selected,
                      s.fs.sel_idx,    s.d_nsel,          s.d_nrawc,         s.d_cand_id,      s.d_cand_corners, s.d_out_count,    s.d_out_ids,     s.d_out_corners,
-                     s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp};
+                     s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp, s.d_out_board};
     for (void* p : dptrs)
         if (p) cudaFree(p);
-    void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp};
+    void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp, s.h_out_board};
     for (void* p : hptrs)
         if (p) cudaFreeHost(p);
     for (int i = 0; i <= ST_COUNT; i++)
@@ -464,7 +476,8 @@ extern "C" int fid_destroy(fid_detector* h) {
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();
     for (int i = 0; i < MAX_SLOTS; i++) free_slot(h->slot[i]);
-    void* ptrs[] = {h->d_prune, h->d_dict, h->d_pf[0], h->d_pf[1], h->d_lut_prev, h->d_lut_next, h->d_subpix_masks, h->d_override_ids, h->d_override_lens, h->d_pose_ids, h->d_pose_corners, h->d_pose_out, h->d_hyp_list};
+    void* ptrs[] = {h->d_prune, h->d_dict, h->d_pf[0], h->d_pf[1], h->d_lut_prev, h->d_lut_next, h->d_subpix_masks, h->d_override_ids, h->d_override_lens, h->d_pose_ids, h->d_pose_corners, h->d_pose_out, h->d_hyp_list,
+                     h->d_board_off, h->d_board_keys, h->d_board_marker, h->d_board_obj, h->d_board_count, h->d_board_list};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     for (int i = 0; i < 2; i++)
@@ -537,6 +550,23 @@ static inline void launch_prio(void (*kernel)(KArgs...), dim3 grid, dim3 block, 
 
 
 // Enqueue the whole pipeline for `nf` frames resident in d_bgr (geometry g) on stream `st`.
+static BoardPoseArgs board_args(const fid_detector* h, const int32_t* count, const int32_t* ids, const float* corners, int max_markers, const fid_camera* cam,
+                                fid_board_pose* out) {
+    BoardPoseArgs a{};
+    a.max_markers = max_markers;
+    a.n_boards = h->n_boards;
+    a.count = count;
+    a.ids = ids;
+    a.corners = corners;
+    a.board_off = h->d_board_off;
+    a.board_keys = h->d_board_keys;
+    a.board_marker = h->d_board_marker;
+    a.board_obj = h->d_board_obj;
+    a.cam = make_camera(cam);
+    a.out = out;
+    return a;
+}
+
 static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, const FrameGeom& g, const uint8_t* d_bgr, const fid_camera* cam, double fiducial_len,
                             int n_override, int stop_after /* -1 = all */, const Slot* prev = nullptr) {
     const DevParams& P = h->P;
@@ -829,19 +859,25 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         launch_prio(k_pose_hypotheses, dim3(nf), dim3(POSE_HYP_THREADS), 0, st, 5, a);
         launches++;
     }
+    if (h->n_boards && cam) {  // opt-in: one pose per (frame, board) over the markers k_finish wrote (fid_set_boards)
+        launch_prio(k_board_pose, dim3(nf * h->n_boards), dim3(FID_BOARD_LANES), 0, st, 5,
+                    board_args(h, s.d_out_count, s.d_out_ids, s.d_out_corners, h->max_markers, cam, s.d_out_board));
+        launches++;
+    }
     CK(cudaEventRecord(s.ev[ST_D2H], st));
     h->counters[6] += launches;
     CK(cudaGetLastError());
     return FID_OK;
 }
 
-static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose, bool with_hyp) {
+static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose, bool with_hyp, bool with_board) {
     const size_t M = (size_t)nf * h->max_markers;
     CK(cudaMemcpyAsync(s.h_out_count, s.d_out_count, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_out_ids, s.d_out_ids, sizeof(int32_t) * M, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_out_corners, s.d_out_corners, sizeof(float) * 8 * M, cudaMemcpyDeviceToHost, st));
     if (with_pose) CK(cudaMemcpyAsync(s.h_out_tf, s.d_out_tf, sizeof(fid_transform) * M, cudaMemcpyDeviceToHost, st));
     if (with_hyp) CK(cudaMemcpyAsync(s.h_out_hyp, s.d_out_hyp, sizeof(struct fid_pose_hypotheses) * M, cudaMemcpyDeviceToHost, st));
+    if (with_board) CK(cudaMemcpyAsync(s.h_out_board, s.d_out_board, sizeof(fid_board_pose) * nf * h->n_boards, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_counters, s.d_counters, sizeof(Counters), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_nsel, s.d_nsel, sizeof(int) * nf, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_nrawc, s.d_nrawc, sizeof(int) * nf, cudaMemcpyDeviceToHost, st));
@@ -851,7 +887,7 @@ static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool w
 }
 
 static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* tfs, bool first_chunk,
-                   struct fid_pose_hypotheses* hyps = nullptr) {
+                   struct fid_pose_hypotheses* hyps = nullptr, fid_board_pose* boards = nullptr) {
     CK(cudaEventSynchronize(s.done));
     int status = FID_OK;
     if (s.h_counters->overflow) status = FID_ERR_CAPACITY;
@@ -867,6 +903,7 @@ static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* c
         if (tfs) memcpy(tfs + (size_t)f * max_markers, s.h_out_tf + (size_t)f * h->max_markers, sizeof(fid_transform) * n);
         if (hyps) memcpy(hyps + (size_t)f * max_markers, s.h_out_hyp + (size_t)f * h->max_markers, sizeof(struct fid_pose_hypotheses) * n);
     }
+    if (boards) memcpy(boards, s.h_out_board, sizeof(fid_board_pose) * nf * h->n_boards);
     // statistics
     float ms = 0;
     static const int order[] = {ST_THRESH, ST_MASKS, ST_WALK, ST_EMIT, ST_APPROX, ST_GROUP, ST_IDENT, ST_SUBPIX_POSE, ST_D2H, ST_COUNT};
@@ -925,6 +962,16 @@ static void end_last_hypotheses(fid_detector* h, bool hyp, const int32_t* counts
     h->last_hyp_valid = true;
 }
 
+// The same for the board poses (fid_last_board_poses), dense [n_frames][n_boards].
+static fid_board_pose* begin_last_boards(fid_detector* h, bool board, int n_frames) {
+    h->last_board_valid = false;
+    if (!board) return nullptr;
+    h->last_board_frames = n_frames;
+    h->last_board_n = h->n_boards;
+    h->last_board.resize((size_t)n_frames * h->n_boards);
+    return h->last_board.data();
+}
+
 extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
                                      const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
                                      int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms) {
@@ -942,6 +989,8 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
     const int n_chunks = (n_frames + B - 1) / B;
     const bool hyp = h->pose_hyp && cam;
     struct fid_pose_hypotheses* hyps = begin_last_hypotheses(h, hyp, n_frames, max_markers);
+    const bool brd = h->n_boards && cam;
+    fid_board_pose* boards = begin_last_boards(h, brd, n_frames);
     h->counters[6] = 0;
     h->stage_ms[ST_H2D] = 0;
     // software pipeline over chunks: up to n_slots chunks in flight, each on its own stream; results of
@@ -994,7 +1043,7 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
             }
             rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, c > 0 ? &h->slot[(c - 1) % NS] : nullptr);
             if (rc != FID_OK) return rc;
-            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp);
+            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp, brd);
             if (rc != FID_OK) return rc;
             h->last_frames = nf;
         }
@@ -1004,11 +1053,12 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
             const int nf = std::min(B, n_frames - pc * B);
             rc = collect(h, s, nf, max_markers, counts + (size_t)pc * B, ids ? ids + (size_t)pc * B * max_markers : nullptr,
                          corners ? corners + (size_t)pc * B * max_markers * 8 : nullptr, (transforms && cam) ? transforms + (size_t)pc * B * max_markers : nullptr, pc == 0,
-                         hyps ? hyps + (size_t)pc * B * max_markers : nullptr);
+                         hyps ? hyps + (size_t)pc * B * max_markers : nullptr, boards ? boards + (size_t)pc * B * h->n_boards : nullptr);
             if (rc != FID_OK) status = rc;
         }
     }
     end_last_hypotheses(h, hyp, counts);
+    h->last_board_valid = brd;
     return status;
 }
 
@@ -1057,7 +1107,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
         const Slot* prev = (h->slots_in_use + c) > 0 ? &h->slot[(si + NS - 1) % NS] : nullptr;
         rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, prev);
         if (rc != FID_OK) return rc;
-        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam);
+        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam, h->n_boards && cam);
         if (rc != FID_OK) return rc;
         h->last_frames = nf;
     }
@@ -1069,6 +1119,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
     pb.h = height;
     pb.pose = cam != nullptr;
     pb.hyp = h->pose_hyp && cam;
+    pb.board = h->n_boards && cam;
     pb.launches = h->counters[6];
     h->pend_count++;
     h->slots_in_use += n_chunks;
@@ -1085,15 +1136,17 @@ extern "C" int fid_collect_batch(fid_detector* h, int max_markers, int32_t* coun
     h->counters[6] = pb.launches;
     h->stage_ms[ST_H2D] = 0;
     struct fid_pose_hypotheses* hyps = begin_last_hypotheses(h, pb.hyp, pb.n_frames, max_markers);
+    fid_board_pose* boards = begin_last_boards(h, pb.board, pb.n_frames);
     for (int c = 0; c < pb.n_chunks; c++) {
         Slot& s = h->slot[(pb.first_slot + c) % NS];
         const int nf = std::min(B, pb.n_frames - c * B);
         const int rc = collect(h, s, nf, max_markers, counts + (size_t)c * B, ids ? ids + (size_t)c * B * max_markers : nullptr,
                                corners ? corners + (size_t)c * B * max_markers * 8 : nullptr, (transforms && pb.pose) ? transforms + (size_t)c * B * max_markers : nullptr, c == 0,
-                               hyps ? hyps + (size_t)c * B * max_markers : nullptr);
+                               hyps ? hyps + (size_t)c * B * max_markers : nullptr, boards ? boards + (size_t)c * B * h->n_boards : nullptr);
         if (rc != FID_OK) status = rc;
     }
     end_last_hypotheses(h, pb.hyp, counts);
+    h->last_board_valid = pb.board;
     h->pend_head = (h->pend_head + 1) % MAX_SLOTS;
     h->pend_count--;
     h->slots_in_use -= pb.n_chunks;
@@ -1188,6 +1241,80 @@ extern "C" int fid_last_pose_hypotheses(fid_detector* h, int max_markers, int* n
         if (h->last_hyp_counts[f] > max_markers) return FID_ERR_CAPACITY;
     for (int f = 0; f < nf; f++)
         memcpy(out + (size_t)f * max_markers, h->last_hyp.data() + (size_t)f * h->last_hyp_stride, sizeof(struct fid_pose_hypotheses) * h->last_hyp_counts[f]);
+    return FID_OK;
+}
+
+extern "C" int fid_set_boards(fid_detector* h, int n_boards, const fid_board* boards) {
+    if (!h || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight read the board tables
+    if (n_boards < 0 || n_boards > FID_MAX_BOARDS || (n_boards > 0 && !boards)) return FID_ERR_INVALID_ARG;
+    std::vector<int32_t> off(1, 0), keys, marker;
+    std::vector<float> obj;
+    for (int b = 0; b < n_boards; b++) {
+        const fid_board& B = boards[b];
+        if (B.n_markers < 1 || B.n_markers > 4096 || !B.ids || !B.obj_points) return FID_ERR_INVALID_ARG;
+        for (int i = 0; i < B.n_markers * 12; i++)
+            if (!std::isfinite(B.obj_points[i])) return FID_ERR_INVALID_ARG;
+        std::vector<int32_t> ord(B.n_markers);
+        for (int i = 0; i < B.n_markers; i++) ord[i] = i;
+        std::sort(ord.begin(), ord.end(), [&](int x, int y) { return B.ids[x] < B.ids[y]; });
+        for (int i = 0; i < B.n_markers; i++) {
+            if (i > 0 && B.ids[ord[i]] == B.ids[ord[i - 1]]) return FID_ERR_INVALID_ARG;  // a repeated id within one board
+            keys.push_back(B.ids[ord[i]]);
+            marker.push_back(ord[i]);
+        }
+        obj.insert(obj.end(), B.obj_points, B.obj_points + (size_t)B.n_markers * 12);
+        off.push_back((int32_t)keys.size());
+    }
+    CK(cudaSetDevice(h->device));
+    for (void* p : {(void*)h->d_board_off, (void*)h->d_board_keys, (void*)h->d_board_marker, (void*)h->d_board_obj})
+        if (p) cudaFree(p);
+    h->d_board_off = h->d_board_keys = h->d_board_marker = nullptr;
+    h->d_board_obj = nullptr;
+    h->n_boards = 0;
+    if (n_boards == 0) return FID_OK;
+    int rc;
+    const size_t M = (size_t)h->max_batch * FID_MAX_BOARDS;
+    for (int i = 0; i < h->n_slots; i++) {  // (a failed allocation leaves the boards off; the next call completes it)
+        Slot& s = h->slot[i];
+        if (!s.d_out_board && (rc = dalloc(&s.d_out_board, M)) != FID_OK) return rc;
+        if (!s.h_out_board && (rc = halloc(&s.h_out_board, M)) != FID_OK) return rc;
+    }
+    if (!h->d_board_list && (rc = dalloc(&h->d_board_list, FID_MAX_BOARDS)) != FID_OK) return rc;
+    if (!h->d_board_count && (rc = dalloc(&h->d_board_count, 1)) != FID_OK) return rc;
+    if ((rc = dalloc(&h->d_board_off, off.size())) != FID_OK || (rc = dalloc(&h->d_board_keys, keys.size())) != FID_OK ||
+        (rc = dalloc(&h->d_board_marker, marker.size())) != FID_OK || (rc = dalloc(&h->d_board_obj, obj.size())) != FID_OK)
+        return rc;
+    CK(cudaMemcpy(h->d_board_off, off.data(), sizeof(int32_t) * off.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_board_keys, keys.data(), sizeof(int32_t) * keys.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_board_marker, marker.data(), sizeof(int32_t) * marker.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_board_obj, obj.data(), sizeof(float) * obj.size(), cudaMemcpyHostToDevice));
+    h->n_boards = n_boards;
+    return FID_OK;
+}
+
+extern "C" int fid_estimate_board_poses(fid_detector* h, int n, const int32_t* ids, const float* corners, const fid_camera* cam, fid_board_pose* out) {
+    if (!h || n < 0 || n > FID_MAX_MARKERS || !cam || !out || (n > 0 && (!ids || !corners)) || h->n_boards == 0) return FID_ERR_INVALID_ARG;
+    CK(cudaSetDevice(h->device));
+    if (n > 0) {
+        CK(cudaMemcpyAsync(h->d_pose_ids, ids, sizeof(int32_t) * n, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(h->d_pose_corners, corners, sizeof(float) * 8 * n, cudaMemcpyHostToDevice, h->stream));
+    }
+    CK(cudaMemcpyAsync(h->d_board_count, &n, sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+    k_board_pose<<<h->n_boards, FID_BOARD_LANES, 0, h->stream>>>(board_args(h, h->d_board_count, h->d_pose_ids, h->d_pose_corners, n, cam, h->d_board_list));
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, h->d_board_list, sizeof(fid_board_pose) * h->n_boards, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return FID_OK;
+}
+
+extern "C" int fid_last_board_poses(fid_detector* h, int max_boards, int* n_frames, int* n_boards, fid_board_pose* out) {
+    if (!h || !n_frames || !n_boards || max_boards < 0 || !h->last_board_valid) return FID_ERR_INVALID_ARG;
+    const int nf = h->last_board_frames, nb = h->last_board_n;
+    *n_frames = nf;
+    *n_boards = nb;
+    if (!out) return FID_OK;
+    if (max_boards < nb) return FID_ERR_CAPACITY;
+    for (int f = 0; f < nf; f++) memcpy(out + (size_t)f * max_boards, h->last_board.data() + (size_t)f * nb, sizeof(fid_board_pose) * nb);
     return FID_OK;
 }
 

@@ -6,10 +6,13 @@
 //   k_finish      one block per frame: compaction in OpenCV's output order, cornerSubPix (A.8),
 //                 solvePnP(ITERATIVE) + FiducialTransform arithmetic                     (A.9)
 //   k_pose_hypotheses  opt-in, after k_finish: both IPPE_SQUARE solutions per marker (ippe.cuh)
+//   k_board_pose  opt-in, after k_finish (and k_pose_hypotheses): one warp per (frame, board), one solvePnP over every
+//                 detected marker of the board (board_pnp.cuh)
 #pragma once
 #include <cuda_runtime.h>
 
 #include "../../include/fiducials_b200.h"
+#include "board_pnp.cuh"
 #include "common.cuh"
 #include "contour_refine.cuh"
 #include "identify.cuh"
@@ -829,6 +832,67 @@ __global__ void __launch_bounds__(64) k_pose_hypotheses_list(const PoseHypListAr
     PoseHypOut ho;
     solve_marker_hypotheses(a.corners + (size_t)m * 8, a.cam, len, po.rvec, &ho);
     pack_hypotheses(id, ho, a.out + m);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// One pose per board (board_pnp.cuh), an opt-in stage of its own so that k_finish and the default pipeline stay as they are.
+struct BoardPoseArgs {
+    int max_markers, n_boards;
+    const int32_t* count;         // [F]                   k_finish's outputs (or one host list)
+    const int32_t* ids;           // [F][max_markers]
+    const float* corners;         // [F][max_markers][8]
+    const int32_t* board_off;     // [n_boards + 1]        board b = rows board_off[b] .. board_off[b + 1] of the three tables
+    const int32_t* board_keys;    //                       its ids, sorted
+    const int32_t* board_marker;  //                       the marker (row within the board) of each sorted id
+    const float* board_obj;       // [rows][4][3]          object points, in the board's own marker order
+    Camera cam;
+    fid_board_pose* out;          // [F][n_boards]
+};
+
+#define BOARD_POSE_MAX_POINTS (4 * FID_MAX_MARKERS)
+
+// One warp per (frame, board): lanes binary-search the board's sorted ids for 32 detections at a time, a ballot / popc prefix
+// keeps Board::matchImagePoints's order while the matched points are staged in shared memory, then the warp solves the pose.
+__global__ void __launch_bounds__(FID_BOARD_LANES) k_board_pose(const BoardPoseArgs a) {
+    __shared__ float s_obj[BOARD_POSE_MAX_POINTS * 3];
+    __shared__ float s_img[BOARD_POSE_MAX_POINTS * 2];
+    __shared__ double s_mn[BOARD_POSE_MAX_POINTS * 2];
+    const int f = blockIdx.x / a.n_boards, b = blockIdx.x % a.n_boards;
+    const int lane = threadIdx.x;
+    const int n = min(a.count[f], FID_MAX_MARKERS);
+    const int off = a.board_off[b], nb = a.board_off[b + 1] - off;
+    const int32_t* ids = a.ids + (size_t)f * a.max_markers;
+    const float* corners = a.corners + (size_t)f * a.max_markers * 8;
+    int m = 0;
+    for (int j0 = 0; j0 < n; j0 += FID_BOARD_LANES) {
+        const int j = j0 + lane;
+        const int k = j < n ? board_find(a.board_keys + off, nb, ids[j]) : -1;
+        const unsigned hit = __ballot_sync(0xffffffffu, k >= 0);
+        if (k >= 0) {
+            const int pos = m + __popc(hit & ((1u << lane) - 1u));
+            const float* o = a.board_obj + (size_t)(off + a.board_marker[off + k]) * 12;
+            for (int c = 0; c < 12; c++) s_obj[pos * 12 + c] = o[c];
+            for (int c = 0; c < 8; c++) s_img[pos * 8 + c] = corners[(size_t)j * 8 + c];
+        }
+        m += __popc(hit);
+    }
+    __syncwarp();
+    BoardPoseOut po;
+    solve_board_pose(4 * m, s_obj, s_img, s_mn, a.cam, &po);
+    if (lane == 0) {
+        fid_board_pose r;
+        r.board = b;
+        r.status = po.status;
+        r.n_markers = m;
+        r.n_points = po.n_points;
+        for (int k = 0; k < 3; k++) {
+            r.rvec[k] = po.rvec[k];
+            r.tvec[k] = po.tvec[k];
+        }
+        for (int k = 0; k < 4; k++) r.rotation[k] = po.quat[k];
+        r.image_error = po.image_error;
+        a.out[(size_t)f * a.n_boards + b] = r;
+    }
 }
 
 }  // namespace fid

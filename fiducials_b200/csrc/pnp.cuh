@@ -161,52 +161,72 @@ struct Camera {
     double k1, k2, p1, p2, k3;  // plumb_bob, first 5 coefficients (aruco_detect.cpp:317-323)
 };
 
+// cv::projectPoints of one object point (X, Y, Z) with R = Rodrigues(p[0..2]) and t = p[3..5]; uv[2] = (u, v);
+// Jm[2][6] = d(u,v)/d(r,t) if non-null (dRdr = dR/dr of rodrigues_v2m, needed only then).
+FID_HD void project_point(double X, double Y, double Z, const double R[9], const double* dRdr, const double p[6], const Camera& cam, double uv[2],
+                          double (*Jm)[6]) {
+    double x = R[0] * X + R[1] * Y + R[2] * Z + p[3];
+    double y = R[3] * X + R[4] * Y + R[5] * Z + p[4];
+    double z = R[6] * X + R[7] * Y + R[8] * Z + p[5];
+    z = z != 0.0 ? 1.0 / z : 1.0;
+    x *= z;
+    y *= z;
+    const double r2 = x * x + y * y, r4 = r2 * r2, r6 = r4 * r2;
+    const double a1 = 2 * x * y, a2 = r2 + 2 * x * x, a3 = r2 + 2 * y * y;
+    const double cdist = 1 + cam.k1 * r2 + cam.k2 * r4 + cam.k3 * r6;
+    const double xd = x * cdist + cam.p1 * a1 + cam.p2 * a2;
+    const double yd = y * cdist + cam.p1 * a3 + cam.p2 * a1;
+    uv[0] = xd * cam.fx + cam.cx;
+    uv[1] = yd * cam.fy + cam.cy;
+    if (Jm) {
+        // translation part
+        double dxd[6], dyd[6];  // d(x)/dparam, d(y)/dparam for the 6 parameters (r then t)
+        for (int j = 0; j < 3; j++) {
+            const double dx0 = X * dRdr[j * 9 + 0] + Y * dRdr[j * 9 + 1] + Z * dRdr[j * 9 + 2];
+            const double dy0 = X * dRdr[j * 9 + 3] + Y * dRdr[j * 9 + 4] + Z * dRdr[j * 9 + 5];
+            const double dz0 = X * dRdr[j * 9 + 6] + Y * dRdr[j * 9 + 7] + Z * dRdr[j * 9 + 8];
+            dxd[j] = z * (dx0 - x * dz0);
+            dyd[j] = z * (dy0 - y * dz0);
+        }
+        dxd[3] = z;
+        dxd[4] = 0;
+        dxd[5] = -x * z;
+        dyd[3] = 0;
+        dyd[4] = z;
+        dyd[5] = -y * z;
+        for (int j = 0; j < 6; j++) {
+            const double dr2 = 2 * x * dxd[j] + 2 * y * dyd[j];
+            const double dcdist = cam.k1 * dr2 + 2 * cam.k2 * r2 * dr2 + 3 * cam.k3 * r4 * dr2;
+            const double da1 = 2 * (x * dyd[j] + y * dxd[j]);
+            const double dmx = dxd[j] * cdist + x * dcdist + cam.p1 * da1 + cam.p2 * (dr2 + 4 * x * dxd[j]);
+            const double dmy = dyd[j] * cdist + y * dcdist + cam.p1 * (dr2 + 4 * y * dyd[j]) + cam.p2 * da1;
+            Jm[0][j] = cam.fx * dmx;
+            Jm[1][j] = cam.fy * dmy;
+        }
+    }
+}
+
+// cv::undistortPoints of one pixel (u, v) to normalised coordinates xy[2]: 5 fixed-point iterations (its default criteria).
+FID_HD void undistort_point(double u, double v, const Camera& cam, double xy[2]) {
+    const double x0 = (u - cam.cx) / cam.fx, y0 = (v - cam.cy) / cam.fy;
+    double x = x0, y = y0;
+    for (int it = 0; it < 5; it++) {
+        const double r2 = x * x + y * y;
+        const double icd = 1.0 / (1 + ((cam.k3 * r2 + cam.k2) * r2 + cam.k1) * r2);
+        const double dx = 2 * cam.p1 * x * y + cam.p2 * (r2 + 2 * x * x);
+        const double dy = cam.p1 * (r2 + 2 * y * y) + 2 * cam.p2 * x * y;
+        x = (x0 - dx) * icd;
+        y = (y0 - dy) * icd;
+    }
+    xy[0] = x;
+    xy[1] = y;
+}
+
 // cv::projectPoints for 4 object points; uv[8] = (u0,v0,...); Jm[8][6] = d(u,v)/d(r,t) if non-null.
 FID_HD void project4(const double obj[4][3], const double p[6], const Camera& cam, double uv[8], double (*Jm)[6]) {
     double R[9], dRdr[27];
     rodrigues_v2m(p, R, Jm ? dRdr : nullptr);
-    for (int i = 0; i < 4; i++) {
-        const double X = obj[i][0], Y = obj[i][1], Z = obj[i][2];
-        double x = R[0] * X + R[1] * Y + R[2] * Z + p[3];
-        double y = R[3] * X + R[4] * Y + R[5] * Z + p[4];
-        double z = R[6] * X + R[7] * Y + R[8] * Z + p[5];
-        z = z != 0.0 ? 1.0 / z : 1.0;
-        x *= z;
-        y *= z;
-        const double r2 = x * x + y * y, r4 = r2 * r2, r6 = r4 * r2;
-        const double a1 = 2 * x * y, a2 = r2 + 2 * x * x, a3 = r2 + 2 * y * y;
-        const double cdist = 1 + cam.k1 * r2 + cam.k2 * r4 + cam.k3 * r6;
-        const double xd = x * cdist + cam.p1 * a1 + cam.p2 * a2;
-        const double yd = y * cdist + cam.p1 * a3 + cam.p2 * a1;
-        uv[2 * i] = xd * cam.fx + cam.cx;
-        uv[2 * i + 1] = yd * cam.fy + cam.cy;
-        if (Jm) {
-            // translation part
-            double dxd[6], dyd[6];  // d(x)/dparam, d(y)/dparam for the 6 parameters (r then t)
-            for (int j = 0; j < 3; j++) {
-                const double dx0 = X * dRdr[j * 9 + 0] + Y * dRdr[j * 9 + 1] + Z * dRdr[j * 9 + 2];
-                const double dy0 = X * dRdr[j * 9 + 3] + Y * dRdr[j * 9 + 4] + Z * dRdr[j * 9 + 5];
-                const double dz0 = X * dRdr[j * 9 + 6] + Y * dRdr[j * 9 + 7] + Z * dRdr[j * 9 + 8];
-                dxd[j] = z * (dx0 - x * dz0);
-                dyd[j] = z * (dy0 - y * dz0);
-            }
-            dxd[3] = z;
-            dxd[4] = 0;
-            dxd[5] = -x * z;
-            dyd[3] = 0;
-            dyd[4] = z;
-            dyd[5] = -y * z;
-            for (int j = 0; j < 6; j++) {
-                const double dr2 = 2 * x * dxd[j] + 2 * y * dyd[j];
-                const double dcdist = cam.k1 * dr2 + 2 * cam.k2 * r2 * dr2 + 3 * cam.k3 * r4 * dr2;
-                const double da1 = 2 * (x * dyd[j] + y * dxd[j]);
-                const double dmx = dxd[j] * cdist + x * dcdist + cam.p1 * da1 + cam.p2 * (dr2 + 4 * x * dxd[j]);
-                const double dmy = dyd[j] * cdist + y * dcdist + cam.p1 * (dr2 + 4 * y * dyd[j]) + cam.p2 * da1;
-                Jm[2 * i][j] = cam.fx * dmx;
-                Jm[2 * i + 1][j] = cam.fy * dmy;
-            }
-        }
-    }
+    for (int i = 0; i < 4; i++) project_point(obj[i][0], obj[i][1], obj[i][2], R, dRdr, p, cam, uv + 2 * i, Jm ? Jm + 2 * i : nullptr);
 }
 
 // Gaussian elimination with partial pivoting, N x N, in place; returns false if singular.
@@ -328,42 +348,45 @@ FID_HD void homography4(const double src[4][2], const double dst[4][2], double H
 // Out of line on the device: inlined into k_pose, nvcc 12.9 (sm_90a, NVVM -O3) miscompiles it -- the LM step comes out
 // wrong and the solver stops after one iteration, rvec off by ~5e-3 (the same source inlined elsewhere, built with
 // -Xcicc -O1, or called out of line gives the host result to 1e-14).
+// N = 6 for the pose; N = 8 for the LM refinement of findHomography (board_pnp.cuh).
+template <int N>
 #if defined(__CUDACC__)
 __host__ __device__ __noinline__
 #else
 inline
 #endif
-void solve_sym6(const double Ain[6][6], const double b[6], double x[6]) {
-    double A[6][6];
-    for (int i = 0; i < 6; i++) {
+void solve_sym(const double Ain[N][N], const double b[N], double x[N]) {
+    double A[N][N];
+    for (int i = 0; i < N; i++) {
         x[i] = b[i];
-        for (int j = 0; j < 6; j++) A[i][j] = Ain[i][j];
+        for (int j = 0; j < N; j++) A[i][j] = Ain[i][j];
     }
     // conditioning guard: smallest pivot relative to the largest diagonal entry
     double dmax = 0.0;
-    for (int i = 0; i < 6; i++) dmax = fabs(Ain[i][i]) > dmax ? fabs(Ain[i][i]) : dmax;
-    bool ok = solve_linear<6>(A, x);
+    for (int i = 0; i < N; i++) dmax = fabs(Ain[i][i]) > dmax ? fabs(Ain[i][i]) : dmax;
+    bool ok = solve_linear<N>(A, x);
     if (ok) {
-        for (int i = 0; i < 6; i++)
+        for (int i = 0; i < N; i++)
             if (!(fabs(A[i][i]) > 1e-11 * dmax)) ok = false;  // A now holds U; tiny pivot => near singular
     }
     if (ok) return;
-    double w[6], V[6][6];
-    for (int i = 0; i < 6; i++)
-        for (int j = 0; j < 6; j++) A[i][j] = Ain[i][j];
-    jacobi_eigen<6>(A, w, V);
+    double w[N], V[N][N];
+    for (int i = 0; i < N; i++)
+        for (int j = 0; j < N; j++) A[i][j] = Ain[i][j];
+    jacobi_eigen<N>(A, w, V);
     double thr = 0.0;
-    for (int i = 0; i < 6; i++) thr += fabs(w[i]);
+    for (int i = 0; i < N; i++) thr += fabs(w[i]);
     thr *= 2.220446049250313e-16 * 2;
-    for (int i = 0; i < 6; i++) x[i] = 0.0;
-    for (int k = 0; k < 6; k++) {
+    for (int i = 0; i < N; i++) x[i] = 0.0;
+    for (int k = 0; k < N; k++) {
         if (fabs(w[k]) <= thr) continue;
         double s = 0.0;
-        for (int i = 0; i < 6; i++) s += V[i][k] * b[i];
+        for (int i = 0; i < N; i++) s += V[i][k] * b[i];
         s /= w[k];
-        for (int i = 0; i < 6; i++) x[i] += s * V[i][k];
+        for (int i = 0; i < N; i++) x[i] += s * V[i][k];
     }
 }
+FID_HD void solve_sym6(const double Ain[6][6], const double b[6], double x[6]) { solve_sym<6>(Ain, b, x); }
 
 struct PoseOut {
     double rvec[3], tvec[3];
@@ -387,20 +410,7 @@ FID_HD void solve_marker_pose(const float corners[8], const Camera& cam, float m
     for (int i = 0; i < 8; i++) img[i] = corners[i];
     // 1. normalise + undistort
     double mn[4][2];
-    for (int i = 0; i < 4; i++) {
-        const double x0 = (img[2 * i] - cam.cx) / cam.fx, y0 = (img[2 * i + 1] - cam.cy) / cam.fy;
-        double x = x0, y = y0;
-        for (int it = 0; it < 5; it++) {
-            const double r2 = x * x + y * y;
-            const double icd = 1.0 / (1 + ((cam.k3 * r2 + cam.k2) * r2 + cam.k1) * r2);
-            const double dx = 2 * cam.p1 * x * y + cam.p2 * (r2 + 2 * x * x);
-            const double dy = cam.p1 * (r2 + 2 * y * y) + 2 * cam.p2 * x * y;
-            x = (x0 - dx) * icd;
-            y = (y0 - dy) * icd;
-        }
-        mn[i][0] = x;
-        mn[i][1] = y;
-    }
+    for (int i = 0; i < 4; i++) undistort_point(img[2 * i], img[2 * i + 1], cam, mn[i]);
     // 2-4. planar initialisation (object plane is z=0 with zero centroid => Rt = I, Tt = 0)
     double src[4][2];
     for (int i = 0; i < 4; i++) {

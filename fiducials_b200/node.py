@@ -180,6 +180,39 @@ class Detector:
         _lib.check(self.lib.fid_last_pose_hypotheses(self.h, max_markers, C.byref(nf), C.cast(out, C.c_void_p)), "fid_last_pose_hypotheses")
         return out
 
+    def set_boards(self, boards):
+        """fid_set_boards: a list of fiducials_b200.board.Board (empty = off).  Batches submitted with a camera from now on also
+        solve one pose per (frame, board)."""
+        boards = list(boards)
+        keep = [(np.ascontiguousarray(b.ids, np.int32), np.ascontiguousarray(b.obj_points, np.float32)) for b in boards]
+        arr = (_lib.fid_board * max(len(keep), 1))()
+        for i, (ids, obj) in enumerate(keep):
+            arr[i].n_markers = len(ids)
+            arr[i].ids = ids.ctypes.data
+            arr[i].obj_points = obj.ctypes.data
+        _lib.check(self.lib.fid_set_boards(self.h, len(keep), C.cast(arr, C.c_void_p)), "fid_set_boards")
+        self.n_boards = len(keep)
+
+    def board_poses(self, ids, corners, K, D):
+        """fid_estimate_board_poses: one fid_board_pose per board set, for markers already detected (ids, corners as detect())."""
+        ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+        corners = np.ascontiguousarray(corners, np.float32).reshape(-1, 8)
+        nb = getattr(self, "n_boards", 0)
+        out = (_lib.fid_board_pose * max(nb, 1))()
+        cam = _camera(K, D)
+        _lib.check(self.lib.fid_estimate_board_poses(self.h, len(ids), ids.ctypes.data_as(C.c_void_p), corners.ctypes.data_as(C.c_void_p), C.byref(cam),
+                                                     C.cast(out, C.c_void_p)), "fid_estimate_board_poses")
+        return [out[i] for i in range(nb)]
+
+    def last_board_poses(self):
+        """fid_last_board_poses: records of the batch last returned by detect_pose_batch / collect_batch, a list per frame of
+        one fid_board_pose per board."""
+        nf, nb = C.c_int(0), C.c_int(0)
+        _lib.check(self.lib.fid_last_board_poses(self.h, 0, C.byref(nf), C.byref(nb), None), "fid_last_board_poses")
+        out = (_lib.fid_board_pose * max(nf.value * nb.value, 1))()
+        _lib.check(self.lib.fid_last_board_poses(self.h, nb.value, C.byref(nf), C.byref(nb), C.cast(out, C.c_void_p)), "fid_last_board_poses")
+        return [[out[f * nb.value + b] for b in range(nb.value)] for f in range(nf.value)]
+
     def debug_threshold(self, bgr):
         bgr = np.ascontiguousarray(bgr, np.uint8)
         H, W = bgr.shape[:2]
@@ -229,7 +262,7 @@ class FiducialsNode:
 
     def __init__(self, dictionary=7, fiducial_len=0.14, ignore_fiducials: Iterable[int] = (), fiducial_len_override: Optional[Dict[int, float]] = None,
                  do_pose_estimation=True, device=0, max_width=1920, max_height=1080, max_batch=1, doCornerRefinement=True, cornerRefinementSubPix=True, pose_hypotheses=False,
-                 **detector_params):
+                 boards=(), **detector_params):
         # doCornerRefinement / cornerRefinementSubPix -> cornerRefinementMethod NONE / SUBPIX / CONTOUR (:700-711, configCallback :274-281)
         detector_params.setdefault("cornerRefinementMethod", (1 if cornerRefinementSubPix else 2) if doCornerRefinement else 0)
         self.fiducial_len = float(fiducial_len)  # :615
@@ -242,6 +275,11 @@ class FiducialsNode:
         self.poseHypotheses = bool(pose_hypotheses)
         if self.poseHypotheses:
             self.det.set_pose_hypotheses(True)
+        # one pose per marker board (new, no reference counterpart): with boards (fiducials_b200.board.Board) the pose results carry
+        # an extra attribute `board_poses` = [fid_board_pose record per board, in board order]; their message fields are unchanged
+        self.boards = list(boards)
+        if self.boards:
+            self.det.set_boards(self.boards)
         self.haveCamInfo = False
         self.K = None
         self.D = None
@@ -295,6 +333,7 @@ class FiducialsNode:
         try:
             tfs = self.det.pose(self.ids, self.corners, self.K, self.D, self.fiducial_len, self.fiducialLens)
             hyps = self.det.pose_hypotheses(self.ids, self.corners, self.K, self.D, self.fiducial_len, self.fiducialLens) if self.poseHypotheses else None
+            boards = self.det.board_poses(self.ids, self.corners, self.K, self.D) if self.boards else None
         except _lib.FidError:
             return fta
         if self.vis_msgs:  # :403, :462-478: vision_msgs/Detection2DArray instead of FiducialTransformArray
@@ -305,6 +344,8 @@ class FiducialsNode:
                 vma.detections.append(Detection2D([ObjectHypothesisWithPose(int(t.fiducial_id), math.exp(-2.0 * float(t.object_error)), tuple(t.translation), tuple(t.rotation))]))
             if hyps is not None:
                 vma.pose_hypotheses = self._by_id(hyps)
+            if boards is not None:
+                vma.board_poses = boards
             return vma
         for t in tfs:
             if t.fiducial_id in self.ignoreIds:
@@ -312,6 +353,8 @@ class FiducialsNode:
             fta.transforms.append(_to_msg(t))
         if hyps is not None:
             fta.pose_hypotheses = self._by_id(hyps)
+        if boards is not None:
+            fta.board_poses = boards
         return fta
 
     def _by_id(self, records):
@@ -323,6 +366,7 @@ class FiducialsNode:
             return []
         counts, ids, corners, tfs = self.det.detect_pose_batch(frames, self.K, self.D, self.fiducial_len, self.fiducialLens)
         hyps = self.det.last_pose_hypotheses() if self.poseHypotheses else None
+        boards = self.det.last_board_poses() if self.boards else None
         out = []
         for f in range(len(counts)):
             fta = FiducialTransformArray(header=Header(0, (0, 0), self.frameId), image_seq=first_seq + f)
@@ -332,6 +376,8 @@ class FiducialsNode:
                     fta.transforms.append(_to_msg(t))
             if hyps is not None:
                 fta.pose_hypotheses = self._by_id(hyps[f * MAXM + m] for m in range(int(counts[f])))
+            if boards is not None:
+                fta.board_poses = boards[f]
             out.append(fta)
         return out
 

@@ -174,6 +174,40 @@ int fid_pose_hypotheses(fid_detector* h, int n, const int32_t* ids, const float*
  * FID_ERR_CAPACITY, with nothing written, if a frame of the batch has more markers than max_markers. */
 int fid_last_pose_hypotheses(fid_detector* h, int max_markers, int* n_frames, struct fid_pose_hypotheses* out);
 
+/* One pose per marker board (NEW; the reference publishes per-marker poses only -- fiducial_slam reads a
+ * `multi_error_theshold` for a multi-fiducial pose, map.cpp:127-129, that it never computes).  A board is a known rigid layout of
+ * markers (a docking station, a calibration target, tags on one plate); its pose restates what OpenCV 4.13 users compute with
+ * cv::aruco::Board::matchImagePoints(corners, ids) + cv::solvePnP(SOLVEPNP_ITERATIVE, no extrinsic guess): every detection whose id
+ * is on the board, in detection order, contributes that marker's 4 object points and its 4 corners (a repeated detection
+ * contributes twice), and one solvePnP runs over all of them (planar or 3-D boards; the branch follows the matched points).
+ * image_error is getReprojectionError (aruco_detect.cpp:203-221) over every matched point; rotation is packed as :447-448. */
+#define FID_MAX_BOARDS 16
+typedef struct fid_board {
+    int32_t n_markers;          /* 1..4096, distinct ids */
+    const int32_t* ids;         /* [n_markers] */
+    const float* obj_points;    /* [n_markers][4][3], metres, marker corner order of cv::aruco::Board */
+} fid_board;
+typedef struct fid_board_pose {
+    int32_t board;              /* index into the fid_set_boards array */
+    int32_t status;             /* 1 pose, 0 no board marker detected, -1 non-planar and < 6 points (cv2 raises) */
+    int32_t n_markers, n_points;
+    double rvec[3], tvec[3], rotation[4];   /* rotation = quaternion x y z w */
+    double image_error;         /* mean squared reprojection error, px^2 */
+} fid_board_pose;
+/* Set the boards of the handle (copied; 0 boards = off, the default).  With boards set, every batch submitted with a camera also
+ * solves one pose per (frame, board) on the device, after the per-marker poses, and copies the records back with the other
+ * results; without boards the batch calls launch exactly what they launch otherwise.  FID_ERR_INVALID_ARG for sizes out of range,
+ * a non-finite object point, an id repeated within one board (a detection could not say which marker it is), or while batches
+ * are in flight. */
+int fid_set_boards(fid_detector* h, int n_boards, const fid_board* boards);
+/* Board poses for markers already detected (0 <= n <= FID_MAX_MARKERS; ids / corners as fid_detect returns them), the counterpart
+ * of fid_pose: out[n_boards] in board order.  FID_ERR_INVALID_ARG if no boards are set. */
+int fid_estimate_board_poses(fid_detector* h, int n, const int32_t* ids, const float* corners, const fid_camera* cam, fid_board_pose* out);
+/* Records of the batch most recently returned by fid_collect_batch / fid_detect_pose_batch, dense [n_frames][max_boards] in board
+ * order.  *n_frames, *n_boards = that batch's counts; out may be NULL to query them.  FID_ERR_INVALID_ARG if that batch ran
+ * without boards or without a camera; FID_ERR_CAPACITY, with nothing written, if max_boards < *n_boards. */
+int fid_last_board_poses(fid_detector* h, int max_boards, int* n_frames, int* n_boards, fid_board_pose* out);
+
 /* Pixel format of the frames handed to every entry point that takes `bgr` (default FID_ENC_BGR8).  The
  * reference converts whatever the camera publishes with cv_bridge::toCvCopy(msg, BGR8)
  * (aruco_detect.cpp:348) before detectMarkers turns it into gray again; the library takes the camera's own
