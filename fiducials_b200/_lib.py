@@ -105,6 +105,34 @@ class fid_board_pose(C.Structure):
     ]
 
 
+class fid_charuco_board(C.Structure):
+    """fid_charuco_board: one ChArUco board, as fid_set_charuco_boards takes it."""
+    _fields_ = [
+        ("squares_x", C.c_int32),
+        ("squares_y", C.c_int32),
+        ("square_length", C.c_float),
+        ("marker_length", C.c_float),
+        ("legacy_pattern", C.c_int32),
+        ("ids", C.c_void_p),
+        ("min_markers", C.c_int32),
+        ("check_markers", C.c_int32),
+    ]
+
+
+class fid_charuco_result(C.Structure):
+    """fid_charuco_result: the corners and pose of one (frame, ChArUco board)."""
+    _fields_ = [
+        ("board", C.c_int32),
+        ("n_corners", C.c_int32),
+        ("corner_offset", C.c_int32),
+        ("status", C.c_int32),
+        ("rvec", C.c_double * 3),
+        ("tvec", C.c_double * 3),
+        ("rotation", C.c_double * 4),
+        ("image_error", C.c_double),
+    ]
+
+
 class fid_map_params(C.Structure):
     _fields_ = [
         ("weighting_scale", C.c_double),
@@ -147,7 +175,7 @@ class fid_map_record(C.Structure):
 # every symbol include/fiducials_b200.h declares (tests/test_abi.py checks the list against the header)
 EXPORTS = [
     "fid_strerror", "fid_version", "fid_default_params", "fid_create", "fid_destroy", "fid_set_params", "fid_detect", "fid_pose",
-    "fid_detect_pose_batch", "fid_submit_batch", "fid_collect_batch", "fid_set_pose_hypotheses", "fid_pose_hypotheses", "fid_last_pose_hypotheses", "fid_set_boards", "fid_estimate_board_poses", "fid_last_board_poses", "fid_hint_next", "fid_set_input_encoding", "fid_timer_start", "fid_timer_stop", "fid_host_alloc", "fid_host_free", "fid_device_alloc", "fid_device_free", "fid_memcpy_h2d", "fid_debug_threshold", "fid_debug_time_threshold",
+    "fid_detect_pose_batch", "fid_submit_batch", "fid_collect_batch", "fid_set_pose_hypotheses", "fid_pose_hypotheses", "fid_last_pose_hypotheses", "fid_set_boards", "fid_estimate_board_poses", "fid_last_board_poses", "fid_set_charuco_boards", "fid_detect_charuco", "fid_last_charuco", "fid_hint_next", "fid_set_input_encoding", "fid_timer_start", "fid_timer_stop", "fid_host_alloc", "fid_host_free", "fid_device_alloc", "fid_device_free", "fid_memcpy_h2d", "fid_debug_threshold", "fid_debug_time_threshold",
     "fid_debug_candidates", "fid_last_stage_ms", "fid_last_counters", "fid_map_default_params", "fid_map_create", "fid_map_destroy", "fid_map_clear",
     "fid_map_load", "fid_map_links", "fid_map_add_links", "fid_map_update", "fid_map_update_sequence", "fid_map_update_frames", "fid_map_update_frames_async", "fid_map_sync", "fid_map_entries", "fid_map_export", "fid_map_merge", "fid_map_export_device",
     "fid_map_merge_device", "fid_map_merge_device_async", "fid_map_export_async", "fid_map_stream", "fid_map_merged_entries", "fid_map_adopt_merged", "fid_map_add_fiducial", "fid_map_refine_default_params", "fid_map_refine",
@@ -184,6 +212,9 @@ def load():
     lib.fid_set_boards.argtypes = [vp, i32, vp]
     lib.fid_estimate_board_poses.argtypes = [vp, i32, vp, vp, C.POINTER(fid_camera), vp]
     lib.fid_last_board_poses.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), vp]
+    lib.fid_set_charuco_boards.argtypes = [vp, i32, vp]
+    lib.fid_detect_charuco.argtypes = [vp, vp, i32, i32, sz, i32, vp, vp, C.POINTER(fid_camera), vp, vp, vp]
+    lib.fid_last_charuco.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), vp, vp, vp]
     lib.fid_hint_next.argtypes = [vp, vp]
     lib.fid_set_input_encoding.argtypes = [vp, i32]
     lib.fid_debug_time_threshold.argtypes = [vp, i32, vp, i32, i32, sz, sz, i32, C.POINTER(C.c_float)]

@@ -49,3 +49,48 @@ def grid_board(size: Tuple[int, int], marker_length: float, separation: float, i
         x0, y0 = np.float32(np.float32(k % w) * step), np.float32(np.float32(k // w) * step)
         obj[k] = [[x0, y0, 0], [np.float32(x0 + L), y0, 0], [np.float32(x0 + L), np.float32(y0 + L), 0], [x0, np.float32(y0 + L), 0]]
     return Board(ids, obj)
+
+
+class CharucoBoard:
+    """A ChArUco board as fid_set_charuco_boards takes it, with its layout (cv::aruco::CharucoBoard of OpenCV 4.13): ``obj_points``
+    [n_markers][4][3] and ``chessboard_corners`` [n_corners][3], float32, equal to cv2's getObjPoints() / getChessboardCorners()."""
+
+    def __init__(self, size, square_length, marker_length, ids=None, legacy=False, min_markers=2, check_markers=True):
+        sx, sy = int(size[0]), int(size[1])
+        if sx < 2 or sy < 2 or (sx - 1) * (sy - 1) > 1024:
+            raise ValueError("charuco_board: size must be >= 2 x 2 with at most 1024 chessboard corners")
+        if not 0 < marker_length < square_length:
+            raise ValueError("charuco_board: 0 < marker_length < square_length")
+        if min_markers not in (0, 1, 2):
+            raise ValueError("charuco_board: min_markers must be 0, 1 or 2")
+        n = sx * sy // 2
+        self.size, self.legacy = (sx, sy), bool(legacy)
+        self.square_length, self.marker_length = float(np.float32(square_length)), float(np.float32(marker_length))
+        self.ids = np.arange(n, dtype=np.int32) if ids is None else np.ascontiguousarray(np.asarray(ids).reshape(-1), np.int32)
+        if len(self.ids) != n or len(np.unique(self.ids)) != n:
+            raise ValueError("charuco_board: %d distinct ids needed" % n)
+        self.min_markers, self.check_markers = int(min_markers), bool(check_markers)
+        S, L = np.float32(square_length), np.float32(marker_length)
+        diff = np.float32((S - L) / np.float32(2))
+        obj = []
+        for y in range(sy):
+            for x in range(sx):
+                if (legacy and sy % 2 == 0 and (y + 1) % 2 == x % 2) or (not (legacy and sy % 2 == 0) and y % 2 == x % 2):
+                    continue
+                x0, y0 = np.float32(np.float32(x) * S + diff), np.float32(np.float32(y) * S + diff)
+                obj.append([[x0, y0, 0], [np.float32(x0 + L), y0, 0], [np.float32(x0 + L), np.float32(y0 + L), 0], [x0, np.float32(y0 + L), 0]])
+        self.obj_points = np.array(obj, np.float32).reshape(-1, 4, 3)
+        self.chessboard_corners = np.array([[np.float32(x + 1) * S, np.float32(y + 1) * S, 0] for y in range(sy - 1) for x in range(sx - 1)], np.float32)
+
+    @property
+    def n_corners(self):
+        return (self.size[0] - 1) * (self.size[1] - 1)
+
+    def __repr__(self):
+        return "CharucoBoard(%dx%d, %d corners)" % (self.size[0], self.size[1], self.n_corners)
+
+
+def charuco_board(size, square_length, marker_length, ids=None, legacy=False, min_markers=2, check_markers=True) -> CharucoBoard:
+    """cv::aruco::CharucoBoard(size, squareLength, markerLength, dictionary, ids) with setLegacyPattern(legacy), and the
+    CharucoParameters minMarkers / checkMarkers its detection uses.  size = (columns, rows) of squares."""
+    return CharucoBoard(size, square_length, marker_length, ids, legacy, min_markers, check_markers)

@@ -59,6 +59,9 @@ struct Slot {
     fid_transform* d_out_tf = nullptr;
     struct fid_pose_hypotheses* d_out_hyp = nullptr;  // fid_set_pose_hypotheses: allocated by the first enable
     fid_board_pose* d_out_board = nullptr;             // fid_set_boards: [max_batch][FID_MAX_BOARDS], allocated by the first set
+    fid_charuco_result* d_out_ch = nullptr;            // fid_set_charuco_boards: [max_batch][FID_MAX_CHARUCO_BOARDS]
+    int32_t* d_out_ch_ids = nullptr;                   // [max_batch][ch_slot_cap]
+    float* d_out_ch_xy = nullptr;                      // [max_batch][ch_slot_cap][2]
     // pinned host mirrors
     int32_t* h_out_count = nullptr;
     int32_t* h_out_ids = nullptr;
@@ -66,6 +69,10 @@ struct Slot {
     fid_transform* h_out_tf = nullptr;
     struct fid_pose_hypotheses* h_out_hyp = nullptr;
     fid_board_pose* h_out_board = nullptr;
+    fid_charuco_result* h_out_ch = nullptr;
+    int32_t* h_out_ch_ids = nullptr;
+    float* h_out_ch_xy = nullptr;
+    int ch_slot_cap = 0;
     Counters* h_counters = nullptr;
     int* h_nsel = nullptr;
     int* h_nrawc = nullptr;
@@ -95,7 +102,7 @@ struct fid_detector {
     struct Pending {
         int first_slot, n_chunks, n_frames, w, h;
         int64_t launches;
-        bool pose, hyp, board;
+        bool pose, hyp, board, charuco;
     } pending[MAX_SLOTS]{};
     int pend_head = 0, pend_count = 0, slots_in_use = 0, slot_next = 0;
     cudaStream_t slot_stream[MAX_SLOTS] = {};
@@ -139,6 +146,20 @@ struct fid_detector {
     bool last_board_valid = false;                   // the batch last returned had boards (and a camera)
     int last_board_frames = 0, last_board_n = 0;
     std::vector<fid_board_pose> last_board;          // [last_board_frames][last_board_n]
+    // ChArUco boards (fid_set_charuco_boards / fid_detect_charuco / fid_last_charuco)
+    int n_charuco = 0, charuco_slots = 0;            // 0 = off; slots = corners of all boards
+    CharucoBoardDev* d_ch_boards = nullptr;
+    int32_t *d_ch_keys = nullptr, *d_ch_marker = nullptr, *d_ch_ids = nullptr, *d_ch_near_n = nullptr, *d_ch_near_idx = nullptr, *d_ch_near_corner = nullptr;
+    float *d_ch_obj = nullptr, *d_ch_chess = nullptr, *d_ch_masks = nullptr;
+    int32_t* d_ch_count = nullptr;                   // fid_detect_charuco: the list's length
+    fid_charuco_result* d_ch_list = nullptr;         // fid_detect_charuco outputs
+    int32_t* d_ch_list_ids = nullptr;
+    float* d_ch_list_xy = nullptr;
+    bool last_ch_valid = false;
+    int last_ch_frames = 0, last_ch_n = 0, last_ch_slots = 0;
+    std::vector<fid_charuco_result> last_ch;         // [last_ch_frames][last_ch_n]
+    std::vector<int32_t> last_ch_ids;                // [last_ch_frames][last_ch_slots]
+    std::vector<float> last_ch_xy;
     float stage_ms[ST_COUNT + N_WALK_ROUNDS]{};
     int64_t counters[8]{};
     cudaEvent_t t0 = nullptr, t1 = nullptr;
@@ -323,10 +344,10 @@ static void free_slot(Slot& s) {
                      s.d_raw,         s.d_nraw,          s.fs.quads_tmp,    s.fs.per_tmp,     s.fs.quads,       s.fs.per,         s.fs.close_bits, s.fs.group_id,
                      s.fs.group_members, s.fs.next_in_group, s.fs.group_head, s.fs.group_tail, s.fs.close_count, s.fs.close_idx,   s.fs.close_off,  s.fs.selected,
                      s.fs.sel_idx,    s.d_nsel,          s.d_nrawc,         s.d_cand_id,      s.d_cand_corners, s.d_out_count,    s.d_out_ids,     s.d_out_corners,
-                     s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp, s.d_out_board};
+                     s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp, s.d_out_board, s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy};
     for (void* p : dptrs)
         if (p) cudaFree(p);
-    void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp, s.h_out_board};
+    void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp, s.h_out_board, s.h_out_ch, s.h_out_ch_ids, s.h_out_ch_xy};
     for (void* p : hptrs)
         if (p) cudaFreeHost(p);
     for (int i = 0; i <= ST_COUNT; i++)
@@ -477,7 +498,9 @@ extern "C" int fid_destroy(fid_detector* h) {
     cudaDeviceSynchronize();
     for (int i = 0; i < MAX_SLOTS; i++) free_slot(h->slot[i]);
     void* ptrs[] = {h->d_prune, h->d_dict, h->d_pf[0], h->d_pf[1], h->d_lut_prev, h->d_lut_next, h->d_subpix_masks, h->d_override_ids, h->d_override_lens, h->d_pose_ids, h->d_pose_corners, h->d_pose_out, h->d_hyp_list,
-                     h->d_board_off, h->d_board_keys, h->d_board_marker, h->d_board_obj, h->d_board_count, h->d_board_list};
+                     h->d_board_off, h->d_board_keys, h->d_board_marker, h->d_board_obj, h->d_board_count, h->d_board_list, h->d_ch_boards, h->d_ch_keys,
+                     h->d_ch_marker, h->d_ch_ids, h->d_ch_near_n, h->d_ch_near_idx, h->d_ch_near_corner, h->d_ch_obj, h->d_ch_chess, h->d_ch_masks,
+                     h->d_ch_count, h->d_ch_list, h->d_ch_list_ids, h->d_ch_list_xy};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     for (int i = 0; i < 2; i++)
@@ -564,6 +587,45 @@ static BoardPoseArgs board_args(const fid_detector* h, const int32_t* count, con
     a.board_obj = h->d_board_obj;
     a.cam = make_camera(cam);
     a.out = out;
+    return a;
+}
+
+static CharucoArgs charuco_args(const fid_detector* h, const uint8_t* src, size_t row_stride, size_t frame_stride, int W, int H, const int32_t* count, const int32_t* ids,
+                                const float* corners, int max_markers, const fid_camera* cam, fid_charuco_result* out, int32_t* out_ids, float* out_xy) {
+    CharucoArgs a{};
+    a.src = src;
+    a.row_stride = row_stride;
+    a.frame_stride = frame_stride;
+    a.enc = h->enc;
+    a.W = W;
+    a.H = H;
+    a.max_markers = max_markers;
+    a.count = count;
+    a.ids = ids;
+    a.corners = corners;
+    a.n_boards = h->n_charuco;
+    a.n_slots = h->charuco_slots;
+    a.boards = h->d_ch_boards;
+    a.keys = h->d_ch_keys;
+    a.marker_of = h->d_ch_marker;
+    a.board_ids = h->d_ch_ids;
+    a.obj = h->d_ch_obj;
+    a.chess = h->d_ch_chess;
+    a.near_n = h->d_ch_near_n;
+    a.near_idx = h->d_ch_near_idx;
+    a.near_corner = h->d_ch_near_corner;
+    a.masks = h->d_ch_masks;
+    // cornerSubPix's own clamps of the criteria (MIN(MAX(maxCount, 1), 100), MAX(epsilon, 0)^2); the detector's window is used
+    // where no nearest marker is detected, within the 1..10 the mask table covers
+    a.win_default = std::max(1, std::min(FID_CHARUCO_MAX_WIN, h->params.cornerRefinementWinSize));
+    a.max_iters = std::max(1, std::min(100, h->params.cornerRefinementMaxIterations));
+    const double eps = std::max(h->params.cornerRefinementMinAccuracy, 0.0);
+    a.eps_sq = eps * eps;
+    a.has_cam = cam ? 1 : 0;
+    a.cam = make_camera(cam);
+    a.out = out;
+    a.out_ids = out_ids;
+    a.out_xy = out_xy;
     return a;
 }
 
@@ -864,13 +926,19 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
                     board_args(h, s.d_out_count, s.d_out_ids, s.d_out_corners, h->max_markers, cam, s.d_out_board));
         launches++;
     }
+    if (h->n_charuco) {  // opt-in: ChArUco corners (and pose with a camera) per (frame, board) (fid_set_charuco_boards)
+        launch_prio(k_charuco, dim3(nf * h->n_charuco), dim3(CHARUCO_THREADS), CHARUCO_SMEM, st, 5,
+                    charuco_args(h, d_bgr, g.bgr_row_stride, g.bgr_frame_stride, g.W, g.H, s.d_out_count, s.d_out_ids, s.d_out_corners, h->max_markers, cam,
+                                 s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy));
+        launches++;
+    }
     CK(cudaEventRecord(s.ev[ST_D2H], st));
     h->counters[6] += launches;
     CK(cudaGetLastError());
     return FID_OK;
 }
 
-static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose, bool with_hyp, bool with_board) {
+static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose, bool with_hyp, bool with_board, bool with_charuco) {
     const size_t M = (size_t)nf * h->max_markers;
     CK(cudaMemcpyAsync(s.h_out_count, s.d_out_count, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_out_ids, s.d_out_ids, sizeof(int32_t) * M, cudaMemcpyDeviceToHost, st));
@@ -878,6 +946,11 @@ static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool w
     if (with_pose) CK(cudaMemcpyAsync(s.h_out_tf, s.d_out_tf, sizeof(fid_transform) * M, cudaMemcpyDeviceToHost, st));
     if (with_hyp) CK(cudaMemcpyAsync(s.h_out_hyp, s.d_out_hyp, sizeof(struct fid_pose_hypotheses) * M, cudaMemcpyDeviceToHost, st));
     if (with_board) CK(cudaMemcpyAsync(s.h_out_board, s.d_out_board, sizeof(fid_board_pose) * nf * h->n_boards, cudaMemcpyDeviceToHost, st));
+    if (with_charuco) {
+        CK(cudaMemcpyAsync(s.h_out_ch, s.d_out_ch, sizeof(fid_charuco_result) * nf * h->n_charuco, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(s.h_out_ch_ids, s.d_out_ch_ids, sizeof(int32_t) * nf * h->charuco_slots, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(s.h_out_ch_xy, s.d_out_ch_xy, sizeof(float) * 2 * nf * h->charuco_slots, cudaMemcpyDeviceToHost, st));
+    }
     CK(cudaMemcpyAsync(s.h_counters, s.d_counters, sizeof(Counters), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_nsel, s.d_nsel, sizeof(int) * nf, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_nrawc, s.d_nrawc, sizeof(int) * nf, cudaMemcpyDeviceToHost, st));
@@ -887,7 +960,7 @@ static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool w
 }
 
 static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* tfs, bool first_chunk,
-                   struct fid_pose_hypotheses* hyps = nullptr, fid_board_pose* boards = nullptr) {
+                   struct fid_pose_hypotheses* hyps = nullptr, fid_board_pose* boards = nullptr, int ch_first = -1) {
     CK(cudaEventSynchronize(s.done));
     int status = FID_OK;
     if (s.h_counters->overflow) status = FID_ERR_CAPACITY;
@@ -904,6 +977,11 @@ static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* c
         if (hyps) memcpy(hyps + (size_t)f * max_markers, s.h_out_hyp + (size_t)f * h->max_markers, sizeof(struct fid_pose_hypotheses) * n);
     }
     if (boards) memcpy(boards, s.h_out_board, sizeof(fid_board_pose) * nf * h->n_boards);
+    if (ch_first >= 0) {  // frames ch_first .. of the ChArUco records of the batch (fid_last_charuco)
+        memcpy(h->last_ch.data() + (size_t)ch_first * h->last_ch_n, s.h_out_ch, sizeof(fid_charuco_result) * nf * h->last_ch_n);
+        memcpy(h->last_ch_ids.data() + (size_t)ch_first * h->last_ch_slots, s.h_out_ch_ids, sizeof(int32_t) * nf * h->last_ch_slots);
+        memcpy(h->last_ch_xy.data() + (size_t)ch_first * h->last_ch_slots * 2, s.h_out_ch_xy, sizeof(float) * 2 * nf * h->last_ch_slots);
+    }
     // statistics
     float ms = 0;
     static const int order[] = {ST_THRESH, ST_MASKS, ST_WALK, ST_EMIT, ST_APPROX, ST_GROUP, ST_IDENT, ST_SUBPIX_POSE, ST_D2H, ST_COUNT};
@@ -972,6 +1050,18 @@ static fid_board_pose* begin_last_boards(fid_detector* h, bool board, int n_fram
     return h->last_board.data();
 }
 
+// The same for the ChArUco records and corners (fid_last_charuco).
+static void begin_last_charuco(fid_detector* h, bool ch, int n_frames) {
+    h->last_ch_valid = false;
+    if (!ch) return;
+    h->last_ch_frames = n_frames;
+    h->last_ch_n = h->n_charuco;
+    h->last_ch_slots = h->charuco_slots;
+    h->last_ch.resize((size_t)n_frames * h->n_charuco);
+    h->last_ch_ids.resize((size_t)n_frames * h->charuco_slots);
+    h->last_ch_xy.resize((size_t)n_frames * h->charuco_slots * 2);
+}
+
 extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
                                      const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
                                      int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms) {
@@ -991,6 +1081,8 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
     struct fid_pose_hypotheses* hyps = begin_last_hypotheses(h, hyp, n_frames, max_markers);
     const bool brd = h->n_boards && cam;
     fid_board_pose* boards = begin_last_boards(h, brd, n_frames);
+    const bool chr = h->n_charuco > 0;
+    begin_last_charuco(h, chr, n_frames);
     h->counters[6] = 0;
     h->stage_ms[ST_H2D] = 0;
     // software pipeline over chunks: up to n_slots chunks in flight, each on its own stream; results of
@@ -1043,7 +1135,7 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
             }
             rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, c > 0 ? &h->slot[(c - 1) % NS] : nullptr);
             if (rc != FID_OK) return rc;
-            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp, brd);
+            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp, brd, chr);
             if (rc != FID_OK) return rc;
             h->last_frames = nf;
         }
@@ -1053,12 +1145,13 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
             const int nf = std::min(B, n_frames - pc * B);
             rc = collect(h, s, nf, max_markers, counts + (size_t)pc * B, ids ? ids + (size_t)pc * B * max_markers : nullptr,
                          corners ? corners + (size_t)pc * B * max_markers * 8 : nullptr, (transforms && cam) ? transforms + (size_t)pc * B * max_markers : nullptr, pc == 0,
-                         hyps ? hyps + (size_t)pc * B * max_markers : nullptr, boards ? boards + (size_t)pc * B * h->n_boards : nullptr);
+                         hyps ? hyps + (size_t)pc * B * max_markers : nullptr, boards ? boards + (size_t)pc * B * h->n_boards : nullptr, chr ? pc * B : -1);
             if (rc != FID_OK) status = rc;
         }
     }
     end_last_hypotheses(h, hyp, counts);
     h->last_board_valid = brd;
+    h->last_ch_valid = chr;
     return status;
 }
 
@@ -1107,7 +1200,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
         const Slot* prev = (h->slots_in_use + c) > 0 ? &h->slot[(si + NS - 1) % NS] : nullptr;
         rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, prev);
         if (rc != FID_OK) return rc;
-        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam, h->n_boards && cam);
+        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam, h->n_boards && cam, h->n_charuco > 0);
         if (rc != FID_OK) return rc;
         h->last_frames = nf;
     }
@@ -1120,6 +1213,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
     pb.pose = cam != nullptr;
     pb.hyp = h->pose_hyp && cam;
     pb.board = h->n_boards && cam;
+    pb.charuco = h->n_charuco > 0;
     pb.launches = h->counters[6];
     h->pend_count++;
     h->slots_in_use += n_chunks;
@@ -1137,16 +1231,19 @@ extern "C" int fid_collect_batch(fid_detector* h, int max_markers, int32_t* coun
     h->stage_ms[ST_H2D] = 0;
     struct fid_pose_hypotheses* hyps = begin_last_hypotheses(h, pb.hyp, pb.n_frames, max_markers);
     fid_board_pose* boards = begin_last_boards(h, pb.board, pb.n_frames);
+    begin_last_charuco(h, pb.charuco, pb.n_frames);
     for (int c = 0; c < pb.n_chunks; c++) {
         Slot& s = h->slot[(pb.first_slot + c) % NS];
         const int nf = std::min(B, pb.n_frames - c * B);
         const int rc = collect(h, s, nf, max_markers, counts + (size_t)c * B, ids ? ids + (size_t)c * B * max_markers : nullptr,
                                corners ? corners + (size_t)c * B * max_markers * 8 : nullptr, (transforms && pb.pose) ? transforms + (size_t)c * B * max_markers : nullptr, c == 0,
-                               hyps ? hyps + (size_t)c * B * max_markers : nullptr, boards ? boards + (size_t)c * B * h->n_boards : nullptr);
+                               hyps ? hyps + (size_t)c * B * max_markers : nullptr, boards ? boards + (size_t)c * B * h->n_boards : nullptr,
+                               pb.charuco ? c * B : -1);
         if (rc != FID_OK) status = rc;
     }
     end_last_hypotheses(h, pb.hyp, counts);
     h->last_board_valid = pb.board;
+    h->last_ch_valid = pb.charuco;
     h->pend_head = (h->pend_head + 1) % MAX_SLOTS;
     h->pend_count--;
     h->slots_in_use -= pb.n_chunks;
@@ -1315,6 +1412,151 @@ extern "C" int fid_last_board_poses(fid_detector* h, int max_boards, int* n_fram
     if (!out) return FID_OK;
     if (max_boards < nb) return FID_ERR_CAPACITY;
     for (int f = 0; f < nf; f++) memcpy(out + (size_t)f * max_boards, h->last_board.data() + (size_t)f * nb, sizeof(fid_board_pose) * nb);
+    return FID_OK;
+}
+
+extern "C" int fid_set_charuco_boards(fid_detector* h, int n_boards, const fid_charuco_board* boards) {
+    if (!h || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight read the board tables
+    if (n_boards < 0 || n_boards > FID_MAX_CHARUCO_BOARDS || (n_boards > 0 && !boards)) return FID_ERR_INVALID_ARG;
+    std::vector<CharucoBoardDev> bd;
+    std::vector<int32_t> keys, marker, ids, near_n, near_idx, near_corner;
+    std::vector<float> obj, chess;
+    for (int b = 0; b < n_boards; b++) {
+        const fid_charuco_board& C = boards[b];
+        const int sx = C.squares_x, sy = C.squares_y;
+        if (sx < 2 || sy < 2 || sx > FID_MAX_CHARUCO_CORNERS + 1 || sy > FID_MAX_CHARUCO_CORNERS + 1 || (sx - 1) * (sy - 1) > FID_MAX_CHARUCO_CORNERS) return FID_ERR_INVALID_ARG;
+        if (!(C.square_length > 0) || !(C.marker_length > 0) || !(C.marker_length < C.square_length) || !std::isfinite(C.square_length)) return FID_ERR_INVALID_ARG;
+        if (C.min_markers < 0 || C.min_markers > 2) return FID_ERR_INVALID_ARG;  // cv2 asserts outside 0..2
+        const int nm = charuco_n_markers(sx, sy), nc = charuco_n_corners(sx, sy);
+        if (nm > h->P.n_markers) return FID_ERR_INVALID_ARG;  // more markers than the dictionary has
+        CharucoBoardDev d{nm, nc, (int)ids.size(), (int)near_n.size(), C.min_markers, C.check_markers ? 1 : 0};
+        std::vector<int32_t> bid(nm);
+        for (int i = 0; i < nm; i++) bid[i] = C.ids ? C.ids[i] : i;
+        std::vector<int32_t> ord(nm);
+        for (int i = 0; i < nm; i++) ord[i] = i;
+        std::sort(ord.begin(), ord.end(), [&](int x, int y) { return bid[x] < bid[y]; });
+        for (int i = 0; i < nm; i++) {
+            if (i > 0 && bid[ord[i]] == bid[ord[i - 1]]) return FID_ERR_INVALID_ARG;  // a repeated id within one board
+            keys.push_back(bid[ord[i]]);
+            marker.push_back(ord[i]);
+        }
+        ids.insert(ids.end(), bid.begin(), bid.end());
+        const size_t o0 = obj.size(), c0 = chess.size(), n0 = near_n.size();
+        obj.resize(o0 + (size_t)nm * 12);
+        chess.resize(c0 + (size_t)nc * 3);
+        near_n.resize(n0 + nc);
+        near_idx.resize(2 * (n0 + nc));
+        near_corner.resize(2 * (n0 + nc));
+        if (!charuco_layout(sx, sy, C.square_length, C.marker_length, C.legacy_pattern != 0, obj.data() + o0, chess.data() + c0, near_n.data() + n0,
+                            near_idx.data() + 2 * n0, near_corner.data() + 2 * n0))
+            return FID_ERR_INVALID_ARG;
+        bd.push_back(d);
+    }
+    CK(cudaSetDevice(h->device));
+    CK(cudaDeviceSynchronize());
+    for (void* p : {(void*)h->d_ch_boards, (void*)h->d_ch_keys, (void*)h->d_ch_marker, (void*)h->d_ch_ids, (void*)h->d_ch_near_n, (void*)h->d_ch_near_idx,
+                    (void*)h->d_ch_near_corner, (void*)h->d_ch_obj, (void*)h->d_ch_chess})
+        if (p) cudaFree(p);
+    h->d_ch_boards = nullptr;
+    h->d_ch_keys = h->d_ch_marker = h->d_ch_ids = h->d_ch_near_n = h->d_ch_near_idx = h->d_ch_near_corner = nullptr;
+    h->d_ch_obj = h->d_ch_chess = nullptr;
+    h->n_charuco = 0;
+    h->charuco_slots = 0;
+    if (n_boards == 0) return FID_OK;
+    const int slots = (int)near_n.size();
+    int rc;
+    for (int i = 0; i < h->n_slots; i++) {  // (a failed allocation leaves the boards off; the next call completes it)
+        Slot& s = h->slot[i];
+        if (!s.d_out_ch && (rc = dalloc(&s.d_out_ch, (size_t)h->max_batch * FID_MAX_CHARUCO_BOARDS)) != FID_OK) return rc;
+        if (!s.h_out_ch && (rc = halloc(&s.h_out_ch, (size_t)h->max_batch * FID_MAX_CHARUCO_BOARDS)) != FID_OK) return rc;
+        if (s.ch_slot_cap < slots) {
+            for (void* p : {(void*)s.d_out_ch_ids, (void*)s.d_out_ch_xy})
+                if (p) cudaFree(p);
+            for (void* p : {(void*)s.h_out_ch_ids, (void*)s.h_out_ch_xy})
+                if (p) cudaFreeHost(p);
+            s.d_out_ch_ids = nullptr;
+            s.d_out_ch_xy = s.h_out_ch_xy = nullptr;
+            s.h_out_ch_ids = nullptr;
+            s.ch_slot_cap = 0;
+            const size_t M = (size_t)h->max_batch * slots;
+            if ((rc = dalloc(&s.d_out_ch_ids, M)) != FID_OK || (rc = dalloc(&s.d_out_ch_xy, 2 * M)) != FID_OK || (rc = halloc(&s.h_out_ch_ids, M)) != FID_OK ||
+                (rc = halloc(&s.h_out_ch_xy, 2 * M)) != FID_OK)
+                return rc;
+            s.ch_slot_cap = slots;
+        }
+    }
+    if (!h->d_ch_masks) {
+        std::vector<float> masks(FID_CHARUCO_MASK_FLOATS);
+        charuco_subpix_masks(masks.data());
+        if ((rc = dalloc(&h->d_ch_masks, masks.size())) != FID_OK) return rc;
+        CK(cudaMemcpy(h->d_ch_masks, masks.data(), sizeof(float) * masks.size(), cudaMemcpyHostToDevice));
+        CK(cudaFuncSetAttribute(k_charuco, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CHARUCO_SMEM));
+    }
+    if (!h->d_ch_count && (rc = dalloc(&h->d_ch_count, 1)) != FID_OK) return rc;
+    if (!h->d_ch_list && (rc = dalloc(&h->d_ch_list, FID_MAX_CHARUCO_BOARDS)) != FID_OK) return rc;
+    if (h->d_ch_list_ids) cudaFree(h->d_ch_list_ids);
+    if (h->d_ch_list_xy) cudaFree(h->d_ch_list_xy);
+    h->d_ch_list_ids = nullptr;
+    h->d_ch_list_xy = nullptr;
+    if ((rc = dalloc(&h->d_ch_list_ids, (size_t)slots)) != FID_OK || (rc = dalloc(&h->d_ch_list_xy, (size_t)2 * slots)) != FID_OK) return rc;
+    if ((rc = dalloc(&h->d_ch_boards, bd.size())) != FID_OK || (rc = dalloc(&h->d_ch_keys, keys.size())) != FID_OK || (rc = dalloc(&h->d_ch_marker, marker.size())) != FID_OK ||
+        (rc = dalloc(&h->d_ch_ids, ids.size())) != FID_OK || (rc = dalloc(&h->d_ch_near_n, near_n.size())) != FID_OK ||
+        (rc = dalloc(&h->d_ch_near_idx, near_idx.size())) != FID_OK || (rc = dalloc(&h->d_ch_near_corner, near_corner.size())) != FID_OK ||
+        (rc = dalloc(&h->d_ch_obj, obj.size())) != FID_OK || (rc = dalloc(&h->d_ch_chess, chess.size())) != FID_OK)
+        return rc;
+    CK(cudaMemcpy(h->d_ch_boards, bd.data(), sizeof(CharucoBoardDev) * bd.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_ch_keys, keys.data(), sizeof(int32_t) * keys.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_ch_marker, marker.data(), sizeof(int32_t) * marker.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_ch_ids, ids.data(), sizeof(int32_t) * ids.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_ch_near_n, near_n.data(), sizeof(int32_t) * near_n.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_ch_near_idx, near_idx.data(), sizeof(int32_t) * near_idx.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_ch_near_corner, near_corner.data(), sizeof(int32_t) * near_corner.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_ch_obj, obj.data(), sizeof(float) * obj.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_ch_chess, chess.data(), sizeof(float) * chess.size(), cudaMemcpyHostToDevice));
+    h->n_charuco = n_boards;
+    h->charuco_slots = slots;
+    return FID_OK;
+}
+
+extern "C" int fid_detect_charuco(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int n, const int32_t* ids, const float* corners,
+                                  const fid_camera* cam, fid_charuco_result* results, int32_t* corner_ids, float* corner_xy) {
+    if (!h || !bgr || n < 0 || n > FID_MAX_MARKERS || (n > 0 && (!ids || !corners)) || !results || !corner_ids || !corner_xy || h->n_charuco == 0) return FID_ERR_INVALID_ARG;
+    if (width < 16 || height < 16 || width > h->max_w || height > h->max_h || stride < (size_t)width * h->bpp) return FID_ERR_INVALID_ARG;
+    if (h->pend_count) return FID_ERR_INVALID_ARG;  // slot 0 may belong to a batch in flight
+    CK(cudaSetDevice(h->device));
+    Slot& s = h->slot[0];
+    CK(cudaMemcpy2DAsync(s.d_bgr, (size_t)width * h->bpp, bgr, stride, (size_t)width * h->bpp, height, cudaMemcpyHostToDevice, h->stream));
+    if (n > 0) {
+        CK(cudaMemcpyAsync(h->d_pose_ids, ids, sizeof(int32_t) * n, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(h->d_pose_corners, corners, sizeof(float) * 8 * n, cudaMemcpyHostToDevice, h->stream));
+    }
+    CK(cudaMemcpyAsync(h->d_ch_count, &n, sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+    k_charuco<<<h->n_charuco, CHARUCO_THREADS, CHARUCO_SMEM, h->stream>>>(charuco_args(h, s.d_bgr, (size_t)width * h->bpp, (size_t)width * h->bpp * height, width, height,
+                                                                                      h->d_ch_count, h->d_pose_ids, h->d_pose_corners, FID_MAX_MARKERS, cam, h->d_ch_list,
+                                                                                      h->d_ch_list_ids, h->d_ch_list_xy));
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(results, h->d_ch_list, sizeof(fid_charuco_result) * h->n_charuco, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(corner_ids, h->d_ch_list_ids, sizeof(int32_t) * h->charuco_slots, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(corner_xy, h->d_ch_list_xy, sizeof(float) * 2 * h->charuco_slots, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return FID_OK;
+}
+
+extern "C" int fid_last_charuco(fid_detector* h, int max_slots, int* n_frames, int* n_boards, int* n_slots, fid_charuco_result* results, int32_t* corner_ids,
+                                float* corner_xy) {
+    if (!h || !n_frames || !n_boards || !n_slots || max_slots < 0 || !h->last_ch_valid) return FID_ERR_INVALID_ARG;
+    const int nf = h->last_ch_frames, nb = h->last_ch_n, ns = h->last_ch_slots;
+    *n_frames = nf;
+    *n_boards = nb;
+    *n_slots = ns;
+    if (!results) return FID_OK;
+    if (!corner_ids || !corner_xy) return FID_ERR_INVALID_ARG;
+    if (max_slots < ns) return FID_ERR_CAPACITY;
+    memcpy(results, h->last_ch.data(), sizeof(fid_charuco_result) * nf * nb);
+    for (int f = 0; f < nf; f++) {
+        memcpy(corner_ids + (size_t)f * max_slots, h->last_ch_ids.data() + (size_t)f * ns, sizeof(int32_t) * ns);
+        memcpy(corner_xy + (size_t)f * max_slots * 2, h->last_ch_xy.data() + (size_t)f * ns * 2, sizeof(float) * 2 * ns);
+    }
     return FID_OK;
 }
 

@@ -8,11 +8,13 @@
 //   k_pose_hypotheses  opt-in, after k_finish: both IPPE_SQUARE solutions per marker (ippe.cuh)
 //   k_board_pose  opt-in, after k_finish (and k_pose_hypotheses): one warp per (frame, board), one solvePnP over every
 //                 detected marker of the board (board_pnp.cuh)
+//   k_charuco     opt-in, last: one block per (frame, ChArUco board), its chessboard corners and pose (charuco.cuh)
 #pragma once
 #include <cuda_runtime.h>
 
 #include "../../include/fiducials_b200.h"
 #include "board_pnp.cuh"
+#include "charuco.cuh"
 #include "common.cuh"
 #include "contour_refine.cuh"
 #include "identify.cuh"
@@ -892,6 +894,193 @@ __global__ void __launch_bounds__(FID_BOARD_LANES) k_board_pose(const BoardPoseA
         for (int k = 0; k < 4; k++) r.rotation[k] = po.quat[k];
         r.image_error = po.image_error;
         a.out[(size_t)f * a.n_boards + b] = r;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// ChArUco corners and pose (charuco.cuh), an opt-in stage of its own after every other stage.
+struct CharucoBoardDev {
+    int n_markers, n_corners;
+    int marker_off, corner_off;  // rows of the marker tables / of the corner tables; corner_off is also the board's first output slot
+    int min_markers, check_markers;
+};
+
+struct CharucoArgs {
+    const uint8_t* src;
+    size_t row_stride, frame_stride;
+    int enc, W, H;
+    int max_markers;
+    const int32_t* count;    // [F]                     k_finish's outputs (or one host list)
+    const int32_t* ids;      // [F][max_markers]
+    const float* corners;    // [F][max_markers][8]
+    int n_boards, n_slots;
+    const CharucoBoardDev* boards;
+    const int32_t *keys, *marker_of, *board_ids;  // marker tables, see CharucoView
+    const float* obj;
+    const float* chess;                           // corner tables
+    const int32_t *near_n, *near_idx, *near_corner;
+    const float* masks;      // charuco_subpix_masks
+    int win_default, max_iters;
+    double eps_sq;
+    int has_cam;
+    Camera cam;
+    fid_charuco_result* out;  // [F][n_boards]
+    int32_t* out_ids;         // [F][n_slots]
+    float* out_xy;            // [F][n_slots][2]
+};
+
+#define CHARUCO_THREADS 128
+#define CHARUCO_PTS (4 * FID_MAX_MARKERS > FID_MAX_CHARUCO_CORNERS ? 4 * FID_MAX_MARKERS : FID_MAX_CHARUCO_CORNERS)
+// dynamic shared memory: points of the two solvePnP calls (obj, img, normalised), detection ids and board markers, corner positions,
+// their output slots and the ids in output order
+#define CHARUCO_SMEM (CHARUCO_PTS * (3 * 4 + 2 * 4 + 2 * 8) + FID_MAX_MARKERS * 2 * 4 + FID_MAX_CHARUCO_CORNERS * (2 * 4 + 4 + 4))
+
+__device__ __forceinline__ void charuco_pack(const BoardPoseOut& po, int status, fid_charuco_result* r) {
+    r->status = status;
+    for (int k = 0; k < 3; k++) {
+        r->rvec[k] = status == 1 ? po.rvec[k] : 0.0;
+        r->tvec[k] = status == 1 ? po.tvec[k] : 0.0;
+    }
+    for (int k = 0; k < 4; k++) r->rotation[k] = status == 1 ? po.quat[k] : 0.0;
+    r->image_error = status == 1 ? po.image_error : 0.0;
+}
+
+// One block per (frame, board).  Warp 0 solves the approximate pose over the board's markers (with a camera), threads then take one
+// chessboard corner at a time (position, window, border and minMarkers filters, cornerSubPix), the block runs checkBoard, the
+// corners are compacted in ascending id, and warp 0 solves the board pose.
+__global__ void __launch_bounds__(CHARUCO_THREADS) k_charuco(const CharucoArgs a) {
+    extern __shared__ __align__(16) unsigned char charuco_smem[];
+    double* s_mn = (double*)charuco_smem;
+    float* s_obj = (float*)(s_mn + 2 * CHARUCO_PTS);
+    float* s_img = s_obj + 3 * CHARUCO_PTS;
+    int32_t* s_ids = (int32_t*)(s_img + 2 * CHARUCO_PTS);
+    int32_t* s_k = s_ids + FID_MAX_MARKERS;
+    float* s_xy = (float*)(s_k + FID_MAX_MARKERS);
+    int32_t* s_slot = (int32_t*)(s_xy + 2 * FID_MAX_CHARUCO_CORNERS);
+    int32_t* s_cid = s_slot + FID_MAX_CHARUCO_CORNERS;
+    __shared__ double s_p[6];
+    __shared__ int s_m, s_n;
+    const int f = blockIdx.x / a.n_boards, b = blockIdx.x % a.n_boards;
+    const int tid = threadIdx.x, lane = tid & 31;
+    const CharucoBoardDev bd = a.boards[b];
+    const CharucoView B{bd.n_markers, bd.n_corners, bd.min_markers, bd.check_markers, a.keys + bd.marker_off, a.marker_of + bd.marker_off, a.board_ids + bd.marker_off,
+                        a.obj + (size_t)bd.marker_off * 12, a.chess + (size_t)bd.corner_off * 3, a.near_n + bd.corner_off, a.near_idx + 2 * bd.corner_off,
+                        a.near_corner + 2 * bd.corner_off};
+    const int n = min(a.count[f], FID_MAX_MARKERS);
+    const int32_t* ids = a.ids + (size_t)f * a.max_markers;
+    const float* corners = a.corners + (size_t)f * a.max_markers * 8;
+    for (int j = tid; j < n; j += CHARUCO_THREADS) {
+        s_ids[j] = ids[j];
+        const int k = board_find(B.keys, B.n_markers, ids[j]);
+        s_k[j] = k < 0 ? -1 : B.marker_of[k];
+    }
+    __syncthreads();
+    // 1. approximate pose (matchImagePoints over the markers in detection order, solvePnP)
+    if (a.has_cam && tid < 32) {
+        int m = 0;
+        for (int j0 = 0; j0 < n; j0 += 32) {
+            const int j = j0 + lane;
+            const int k = j < n ? s_k[j] : -1;
+            const unsigned hit = __ballot_sync(0xffffffffu, k >= 0);
+            if (k >= 0) {
+                const int pos = m + __popc(hit & ((1u << lane) - 1u));
+                for (int c = 0; c < 12; c++) s_obj[pos * 12 + c] = B.obj[(size_t)k * 12 + c];
+                for (int c = 0; c < 8; c++) s_img[pos * 8 + c] = corners[(size_t)j * 8 + c];
+            }
+            m += __popc(hit);
+        }
+        __syncwarp();
+        if (m > 0) {
+            BoardPoseOut po;
+            solve_board_pose(4 * m, s_obj, s_img, s_mn, a.cam, &po);
+            if (lane == 0)
+                for (int k = 0; k < 3; k++) {
+                    s_p[k] = po.rvec[k];
+                    s_p[3 + k] = po.tvec[k];
+                }
+        }
+        if (lane == 0) s_m = m;
+    }
+    __syncthreads();
+    const bool any = !a.has_cam || s_m > 0;
+    double p[6], R[9];
+    if (a.has_cam && any) {
+        for (int k = 0; k < 6; k++) p[k] = s_p[k];
+        rodrigues_v2m(p, R, nullptr);
+    }
+    // 2. per corner: position, window, filters, cornerSubPix
+    const FrameImg gray{a.src + (size_t)f * a.frame_stride, a.row_stride, a.enc};
+    for (int i = tid; i < B.n_corners; i += CHARUCO_THREADS) {
+        float xy[2] = {-1.f, -1.f};
+        bool keep = false;
+        if (any) {
+            if (a.has_cam) charuco_project(B, i, R, p, a.cam, xy);
+            else charuco_corner_local(B, i, n, s_ids, corners, xy);
+            keep = charuco_inside(xy, a.W, a.H) && charuco_marker_count(B, i, n, s_ids) >= B.min_markers;
+            if (keep) {
+                const int win = charuco_window(B, i, xy, n, s_ids, corners);
+                float patch[(2 * FID_CHARUCO_MAX_WIN + 3) * (2 * FID_CHARUCO_MAX_WIN + 3)];
+                charuco_refine(gray, a.W, a.H, xy, win < 0 ? a.win_default : win, a.masks, a.max_iters, a.eps_sq, patch);
+            }
+        }
+        s_xy[2 * i] = xy[0];
+        s_xy[2 * i + 1] = xy[1];
+        s_slot[i] = keep ? 1 : 0;
+    }
+    __syncthreads();
+    // 3. checkBoard over the corners kept
+    int bad = 0;
+    if (B.check_markers)
+        for (int i = tid; i < B.n_corners; i += CHARUCO_THREADS)
+            if (s_slot[i] && !charuco_check_corner(B, i, s_xy + 2 * i, n, s_ids, s_k, corners)) bad = 1;
+    bad = __syncthreads_or(bad);
+    // 4. compaction in ascending id
+    if (tid == 0) {
+        int q = 0;
+        for (int i = 0; i < B.n_corners; i++) {
+            const int keep = s_slot[i] && !bad;
+            s_slot[i] = keep ? q : -1;
+            if (keep) s_cid[q++] = i;
+        }
+        s_n = q;
+    }
+    __syncthreads();
+    const int nc = s_n;
+    int32_t* oid = a.out_ids + (size_t)f * a.n_slots + bd.corner_off;
+    float* oxy = a.out_xy + ((size_t)f * a.n_slots + bd.corner_off) * 2;
+    for (int q = tid; q < B.n_corners; q += CHARUCO_THREADS) {
+        if (q < nc) {
+            const int i = s_cid[q];
+            oid[q] = i;
+            oxy[2 * q] = s_img[2 * q] = s_xy[2 * i];
+            oxy[2 * q + 1] = s_img[2 * q + 1] = s_xy[2 * i + 1];
+            for (int k = 0; k < 3; k++) s_obj[3 * q + k] = B.chess[3 * i + k];
+        } else {
+            oid[q] = -1;
+            oxy[2 * q] = oxy[2 * q + 1] = -1.f;
+        }
+    }
+    __syncthreads();
+    // 5. the board pose
+    if (tid < 32) {
+        BoardPoseOut po{};
+        int status = 0;
+        if (bad) status = -3;
+        else if (a.has_cam && nc >= 4) {
+            if (charuco_collinear(B, nc, s_cid)) status = -2;
+            else {
+                solve_board_pose(nc, s_obj, s_img, s_mn, a.cam, &po);
+                status = po.status;  // 1: the chessboard corners lie in z = 0, so the planar branch runs, which always solves
+            }
+        }
+        if (lane == 0) {
+            fid_charuco_result r;
+            r.board = b;
+            r.n_corners = nc;
+            r.corner_offset = bd.corner_off;
+            charuco_pack(po, status, &r);
+            a.out[(size_t)f * a.n_boards + b] = r;
+        }
     }
 }
 

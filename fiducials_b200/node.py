@@ -213,6 +213,59 @@ class Detector:
         _lib.check(self.lib.fid_last_board_poses(self.h, nb.value, C.byref(nf), C.byref(nb), C.cast(out, C.c_void_p)), "fid_last_board_poses")
         return [[out[f * nb.value + b] for b in range(nb.value)] for f in range(nf.value)]
 
+    def set_charuco_boards(self, boards):
+        """fid_set_charuco_boards: a list of fiducials_b200.board.CharucoBoard (empty = off).  Batches submitted from now on also
+        find each board's chessboard corners (and, with a camera, its pose)."""
+        boards = list(boards)
+        arr = (_lib.fid_charuco_board * max(len(boards), 1))()
+        keep = []
+        for i, b in enumerate(boards):
+            ids = np.ascontiguousarray(b.ids, np.int32)
+            keep.append(ids)
+            arr[i].squares_x, arr[i].squares_y = b.size
+            arr[i].square_length, arr[i].marker_length = b.square_length, b.marker_length
+            arr[i].legacy_pattern, arr[i].ids = int(b.legacy), ids.ctypes.data
+            arr[i].min_markers, arr[i].check_markers = b.min_markers, int(b.check_markers)
+        _lib.check(self.lib.fid_set_charuco_boards(self.h, len(boards), C.cast(arr, C.c_void_p)), "fid_set_charuco_boards")
+        self.charuco_boards = boards
+
+    def _charuco_split(self, recs, cids, cxy):
+        out = []
+        for r in recs:
+            o, n = int(r.corner_offset), int(r.n_corners)
+            out.append((r, cids[o:o + n].copy(), cxy[o:o + n].copy()))
+        return out
+
+    def charuco(self, frame, ids, corners, K=None, D=None):
+        """fid_detect_charuco: per ChArUco board set, (fid_charuco_result, corner ids [n], corners [n, 2]) for one frame and markers
+        already detected (ids, corners as detect()).  Without K no pose."""
+        frame = np.ascontiguousarray(frame, np.uint8)
+        H, W = frame.shape[:2]
+        ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+        corners = np.ascontiguousarray(corners, np.float32).reshape(-1, 8)
+        boards = getattr(self, "charuco_boards", [])
+        slots = sum(b.n_corners for b in boards)
+        recs = (_lib.fid_charuco_result * max(len(boards), 1))()
+        cids = np.zeros(max(slots, 1), np.int32)
+        cxy = np.zeros((max(slots, 1), 2), np.float32)
+        cam = None if K is None else C.byref(_camera(K, D))
+        _lib.check(self.lib.fid_detect_charuco(self.h, frame.ctypes.data_as(C.c_void_p), W, H, frame.strides[0], len(ids), ids.ctypes.data_as(C.c_void_p),
+                                               corners.ctypes.data_as(C.c_void_p), cam, C.cast(recs, C.c_void_p), cids.ctypes.data_as(C.c_void_p),
+                                               cxy.ctypes.data_as(C.c_void_p)), "fid_detect_charuco")
+        return self._charuco_split([recs[i] for i in range(len(boards))], cids, cxy)
+
+    def last_charuco(self):
+        """fid_last_charuco: for the batch last returned by detect_pose_batch / collect_batch, a list per frame of
+        (fid_charuco_result, corner ids, corners) per ChArUco board."""
+        nf, nb, ns = C.c_int(0), C.c_int(0), C.c_int(0)
+        _lib.check(self.lib.fid_last_charuco(self.h, 0, C.byref(nf), C.byref(nb), C.byref(ns), None, None, None), "fid_last_charuco")
+        recs = (_lib.fid_charuco_result * max(nf.value * nb.value, 1))()
+        cids = np.zeros((max(nf.value, 1), max(ns.value, 1)), np.int32)
+        cxy = np.zeros((max(nf.value, 1), max(ns.value, 1), 2), np.float32)
+        _lib.check(self.lib.fid_last_charuco(self.h, cids.shape[1], C.byref(nf), C.byref(nb), C.byref(ns), C.cast(recs, C.c_void_p), cids.ctypes.data_as(C.c_void_p),
+                                             cxy.ctypes.data_as(C.c_void_p)), "fid_last_charuco")
+        return [self._charuco_split([recs[f * nb.value + b] for b in range(nb.value)], cids[f], cxy[f]) for f in range(nf.value)]
+
     def debug_threshold(self, bgr):
         bgr = np.ascontiguousarray(bgr, np.uint8)
         H, W = bgr.shape[:2]
@@ -262,7 +315,7 @@ class FiducialsNode:
 
     def __init__(self, dictionary=7, fiducial_len=0.14, ignore_fiducials: Iterable[int] = (), fiducial_len_override: Optional[Dict[int, float]] = None,
                  do_pose_estimation=True, device=0, max_width=1920, max_height=1080, max_batch=1, doCornerRefinement=True, cornerRefinementSubPix=True, pose_hypotheses=False,
-                 boards=(), **detector_params):
+                 boards=(), charuco_boards=(), **detector_params):
         # doCornerRefinement / cornerRefinementSubPix -> cornerRefinementMethod NONE / SUBPIX / CONTOUR (:700-711, configCallback :274-281)
         detector_params.setdefault("cornerRefinementMethod", (1 if cornerRefinementSubPix else 2) if doCornerRefinement else 0)
         self.fiducial_len = float(fiducial_len)  # :615
@@ -280,6 +333,12 @@ class FiducialsNode:
         self.boards = list(boards)
         if self.boards:
             self.det.set_boards(self.boards)
+        # ChArUco boards (new, no reference counterpart): with charuco_boards (fiducials_b200.board.CharucoBoard) the pose results
+        # carry an extra attribute `charuco` = [(fid_charuco_result, corner ids, corners [n, 2]) per board, in board order]
+        self.charucoBoards = list(charuco_boards)
+        if self.charucoBoards:
+            self.det.set_charuco_boards(self.charucoBoards)
+        self._last_frame = None  # the frame of the last imageCallback, for the ChArUco corners of poseEstimateCallback
         self.haveCamInfo = False
         self.K = None
         self.D = None
@@ -313,6 +372,8 @@ class FiducialsNode:
             self.ids, self.corners = self.det.detect(bgr)  # :350
         except _lib.FidError:
             return None  # frame dropped (:389-394)
+        if self.charucoBoards:
+            self._last_frame = np.ascontiguousarray(bgr, np.uint8)
         for i, fid in enumerate(self.ids.tolist()):
             if fid in self.ignoreIds:
                 continue  # :359-364
@@ -334,6 +395,7 @@ class FiducialsNode:
             tfs = self.det.pose(self.ids, self.corners, self.K, self.D, self.fiducial_len, self.fiducialLens)
             hyps = self.det.pose_hypotheses(self.ids, self.corners, self.K, self.D, self.fiducial_len, self.fiducialLens) if self.poseHypotheses else None
             boards = self.det.board_poses(self.ids, self.corners, self.K, self.D) if self.boards else None
+            charuco = self.det.charuco(self._last_frame, self.ids, self.corners, self.K, self.D) if self.charucoBoards and self._last_frame is not None else None
         except _lib.FidError:
             return fta
         if self.vis_msgs:  # :403, :462-478: vision_msgs/Detection2DArray instead of FiducialTransformArray
@@ -346,6 +408,8 @@ class FiducialsNode:
                 vma.pose_hypotheses = self._by_id(hyps)
             if boards is not None:
                 vma.board_poses = boards
+            if charuco is not None:
+                vma.charuco = charuco
             return vma
         for t in tfs:
             if t.fiducial_id in self.ignoreIds:
@@ -355,6 +419,8 @@ class FiducialsNode:
             fta.pose_hypotheses = self._by_id(hyps)
         if boards is not None:
             fta.board_poses = boards
+        if charuco is not None:
+            fta.charuco = charuco
         return fta
 
     def _by_id(self, records):
@@ -367,6 +433,7 @@ class FiducialsNode:
         counts, ids, corners, tfs = self.det.detect_pose_batch(frames, self.K, self.D, self.fiducial_len, self.fiducialLens)
         hyps = self.det.last_pose_hypotheses() if self.poseHypotheses else None
         boards = self.det.last_board_poses() if self.boards else None
+        charuco = self.det.last_charuco() if self.charucoBoards else None
         out = []
         for f in range(len(counts)):
             fta = FiducialTransformArray(header=Header(0, (0, 0), self.frameId), image_seq=first_seq + f)
@@ -378,6 +445,8 @@ class FiducialsNode:
                 fta.pose_hypotheses = self._by_id(hyps[f * MAXM + m] for m in range(int(counts[f])))
             if boards is not None:
                 fta.board_poses = boards[f]
+            if charuco is not None:
+                fta.charuco = charuco[f]
             out.append(fta)
         return out
 

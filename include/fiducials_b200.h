@@ -208,6 +208,51 @@ int fid_estimate_board_poses(fid_detector* h, int n, const int32_t* ids, const f
  * without boards or without a camera; FID_ERR_CAPACITY, with nothing written, if max_boards < *n_boards. */
 int fid_last_board_poses(fid_detector* h, int max_boards, int* n_frames, int* n_boards, fid_board_pose* out);
 
+/* ChArUco boards (NEW): a chessboard with a marker in every white square, as cv::aruco::CharucoBoard(size, squareLength,
+ * markerLength, dictionary, ids) of OpenCV 4.13 lays it out.  Its chessboard corners are found from the detected markers as
+ * cv::aruco::CharucoDetector::detectBoard(image, charucoCorners, charucoIds, markerCorners, markerIds) finds them for markers it is
+ * given (with a camera through an approximate solvePnP over the markers, without one through each marker's local homography;
+ * cornerSubPix with per-corner windows of 1..10 px and the detector's cornerRefinementMaxIterations / MinAccuracy; minMarkers and
+ * checkMarkers), and the board pose is CharucoBoard::matchImagePoints(corners, ids) + cv::solvePnP(SOLVEPNP_ITERATIVE). */
+#define FID_MAX_CHARUCO_BOARDS 16
+#define FID_MAX_CHARUCO_CORNERS 1024 /* per board: (squares_x - 1) (squares_y - 1) */
+typedef struct fid_charuco_board {
+    int32_t squares_x, squares_y;  /* >= 2 each */
+    float square_length, marker_length;  /* metres, 0 < marker_length < square_length */
+    int32_t legacy_pattern;        /* CharucoBoard::setLegacyPattern */
+    const int32_t* ids;            /* [squares_x * squares_y / 2] distinct marker ids, or NULL for 0 .. n - 1 */
+    int32_t min_markers;           /* CharucoParameters::minMarkers, 0..2 (cv2 default 2) */
+    int32_t check_markers;         /* CharucoParameters::checkMarkers (cv2 default 1) */
+} fid_charuco_board;
+typedef struct fid_charuco_result {
+    int32_t board;                 /* index into the fid_set_charuco_boards array */
+    int32_t n_corners;             /* corners found */
+    int32_t corner_offset;         /* first slot of this board in the per-frame corner arrays */
+    int32_t status;                /* 1 pose, 0 no camera or < 4 corners, -2 collinear corners, -3 rejected by checkMarkers (the
+                                      corners are coplanar, so solvePnP's -1 of fid_board_pose cannot occur) */
+    double rvec[3], tvec[3], rotation[4];  /* rotation = quaternion x y z w */
+    double image_error;            /* mean squared reprojection error of the corners, px^2 */
+} fid_charuco_result;
+/* Set the ChArUco boards of the handle (the layout is computed from these numbers; 0 boards = off, the default).  Each board owns
+ * (squares_x - 1)(squares_y - 1) slots of the per-frame corner arrays, board after board; its n_corners first slots hold the
+ * corners in ascending corner id (cv2's order), the others id -1 and (-1, -1).  With boards set, every batch also finds the corners
+ * of each (frame, board) on the device after the other stages, with or without a camera (no pose without one), and copies them
+ * back with the other results; without boards the batch calls launch exactly what they launch otherwise.  FID_ERR_INVALID_ARG for
+ * sizes out of range, repeated ids within a board, more markers than the dictionary has, or while batches are in flight. */
+int fid_set_charuco_boards(fid_detector* h, int n_boards, const fid_charuco_board* boards);
+/* Corners and pose of every ChArUco board set, for one frame (in the fid_set_input_encoding format) and markers already detected
+ * (0 <= n <= FID_MAX_MARKERS; ids / corners as fid_detect returns them): the counterpart of detectBoard(image, markerCorners,
+ * markerIds).  cam may be NULL.  results[n_boards]; corner_ids / corner_xy [total slots] ([2] floats per slot).  No marker: no
+ * corner.  FID_ERR_INVALID_ARG if no boards are set or while batches are in flight. */
+int fid_detect_charuco(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int n, const int32_t* ids, const float* corners,
+                       const fid_camera* cam, fid_charuco_result* results, int32_t* corner_ids, float* corner_xy);
+/* Records and corners of the batch most recently returned by fid_collect_batch / fid_detect_pose_batch: results dense
+ * [n_frames][n_boards], corners dense [n_frames][max_slots].  *n_frames, *n_boards, *n_slots = that batch's counts; results may
+ * be NULL to query them.  FID_ERR_INVALID_ARG if that batch ran without ChArUco boards; FID_ERR_CAPACITY, with nothing written, if
+ * max_slots < *n_slots. */
+int fid_last_charuco(fid_detector* h, int max_slots, int* n_frames, int* n_boards, int* n_slots, fid_charuco_result* results, int32_t* corner_ids,
+                     float* corner_xy);
+
 /* Pixel format of the frames handed to every entry point that takes `bgr` (default FID_ENC_BGR8).  The
  * reference converts whatever the camera publishes with cv_bridge::toCvCopy(msg, BGR8)
  * (aruco_detect.cpp:348) before detectMarkers turns it into gray again; the library takes the camera's own
