@@ -160,6 +160,10 @@ struct fid_detector {
     std::vector<fid_charuco_result> last_ch;         // [last_ch_frames][last_ch_n]
     std::vector<int32_t> last_ch_ids;                // [last_ch_frames][last_ch_slots]
     std::vector<float> last_ch_xy;
+    // recovery of missed board markers (fid_set_marker_refinement / fid_refine_detected_markers)
+    fid_marker_refine_params mrefine{};              // enable = 0: off
+    int32_t* d_mr_i = nullptr;                       // count, n_rejected, n_recovered, overflow, ids, recovered idx, recovered board
+    float* d_mr_f = nullptr;                         // corners [FID_MAX_MARKERS][8], rejected [FID_MAX_REJECTED][8]
     float stage_ms[ST_COUNT + N_WALK_ROUNDS]{};
     int64_t counters[8]{};
     cudaEvent_t t0 = nullptr, t1 = nullptr;
@@ -500,7 +504,7 @@ extern "C" int fid_destroy(fid_detector* h) {
     void* ptrs[] = {h->d_prune, h->d_dict, h->d_pf[0], h->d_pf[1], h->d_lut_prev, h->d_lut_next, h->d_subpix_masks, h->d_override_ids, h->d_override_lens, h->d_pose_ids, h->d_pose_corners, h->d_pose_out, h->d_hyp_list,
                      h->d_board_off, h->d_board_keys, h->d_board_marker, h->d_board_obj, h->d_board_count, h->d_board_list, h->d_ch_boards, h->d_ch_keys,
                      h->d_ch_marker, h->d_ch_ids, h->d_ch_near_n, h->d_ch_near_idx, h->d_ch_near_corner, h->d_ch_obj, h->d_ch_chess, h->d_ch_masks,
-                     h->d_ch_count, h->d_ch_list, h->d_ch_list_ids, h->d_ch_list_xy};
+                     h->d_ch_count, h->d_ch_list, h->d_ch_list_ids, h->d_ch_list_xy, h->d_mr_i, h->d_mr_f};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     for (int i = 0; i < 2; i++)
@@ -1557,6 +1561,98 @@ extern "C" int fid_last_charuco(fid_detector* h, int max_slots, int* n_frames, i
         memcpy(corner_ids + (size_t)f * max_slots, h->last_ch_ids.data() + (size_t)f * ns, sizeof(int32_t) * ns);
         memcpy(corner_xy + (size_t)f * max_slots * 2, h->last_ch_xy.data() + (size_t)f * ns * 2, sizeof(float) * 2 * ns);
     }
+    return FID_OK;
+}
+
+extern "C" int fid_set_marker_refinement(fid_detector* h, const fid_marker_refine_params* params) {
+    if (!h || !params || h->pend_count) return FID_ERR_INVALID_ARG;
+    const fid_marker_refine_params p = *params;
+    if (p.enable && (!(p.min_rep_distance > 0) || !std::isfinite(p.min_rep_distance) || !std::isfinite(p.error_correction_rate))) return FID_ERR_INVALID_ARG;
+    if (p.enable) {  // (a failed allocation leaves the option off; the next enable completes it)
+        CK(cudaSetDevice(h->device));
+        int rc;
+        if (!h->d_mr_i && (rc = dalloc(&h->d_mr_i, 4 + 3 * (size_t)FID_MAX_MARKERS)) != FID_OK) return rc;
+        if (!h->d_mr_f && (rc = dalloc(&h->d_mr_f, 8 * ((size_t)FID_MAX_MARKERS + FID_MAX_REJECTED))) != FID_OK) return rc;
+        CK(cudaFuncSetAttribute(k_marker_refine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MREFINE_SMEM));
+    }
+    h->mrefine = p;
+    h->mrefine.enable = p.enable ? 1 : 0;
+    return FID_OK;
+}
+
+extern "C" int fid_refine_detected_markers(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int n, int32_t* ids, float* corners,
+                                           int max_markers, int n_rejected, const float* rejected, const fid_camera* cam, int* n_out, int32_t* recovered_idx,
+                                           int32_t* recovered_board) {
+    if (!h || !bgr || !n_out || !recovered_idx || !recovered_board || max_markers < 0 || max_markers > FID_MAX_MARKERS || n < 0 || n > max_markers ||
+        (max_markers > 0 && (!ids || !corners)) || n_rejected < 0 || n_rejected > FID_MAX_REJECTED || (n_rejected > 0 && !rejected))
+        return FID_ERR_INVALID_ARG;
+    if (width < 16 || height < 16 || width > h->max_w || height > h->max_h || stride < (size_t)width * h->bpp) return FID_ERR_INVALID_ARG;
+    if (!h->mrefine.enable || h->n_boards + h->n_charuco == 0) return FID_ERR_INVALID_ARG;
+    if (h->pend_count) return FID_ERR_INVALID_ARG;  // slot 0 may belong to a batch in flight
+    CK(cudaSetDevice(h->device));
+    Slot& s = h->slot[0];
+    int32_t* d_count = h->d_mr_i;
+    int32_t* d_ids = h->d_mr_i + 4;
+    int32_t* d_rec_idx = d_ids + FID_MAX_MARKERS;
+    int32_t* d_rec_board = d_rec_idx + FID_MAX_MARKERS;
+    float* d_corners = h->d_mr_f;
+    float* d_rej = h->d_mr_f + 8 * FID_MAX_MARKERS;
+    const int32_t head[4] = {n, n_rejected, 0, 0};
+    CK(cudaMemcpy2DAsync(s.d_bgr, (size_t)width * h->bpp, bgr, stride, (size_t)width * h->bpp, height, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(d_count, head, sizeof(head), cudaMemcpyHostToDevice, h->stream));
+    if (n > 0) {
+        CK(cudaMemcpyAsync(d_ids, ids, sizeof(int32_t) * n, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(d_corners, corners, sizeof(float) * 8 * n, cudaMemcpyHostToDevice, h->stream));
+    }
+    if (n_rejected > 0) CK(cudaMemcpyAsync(d_rej, rejected, sizeof(float) * 8 * n_rejected, cudaMemcpyHostToDevice, h->stream));
+    MarkerRefineArgs a{};
+    a.src = s.d_bgr;
+    a.row_stride = (size_t)width * h->bpp;
+    a.frame_stride = a.row_stride * height;
+    a.enc = h->enc;
+    a.W = width;
+    a.H = height;
+    a.P = h->P;
+    a.dict = h->d_dict;
+    a.subpix_masks = h->d_subpix_masks;
+    a.rp = MarkerRefineParams{h->mrefine.min_rep_distance, h->mrefine.error_correction_rate, h->mrefine.check_all_orders ? 1 : 0};
+    a.n_boards = h->n_boards;
+    a.board_off = h->d_board_off;
+    a.board_keys = h->d_board_keys;
+    a.board_marker = h->d_board_marker;
+    a.board_obj = h->d_board_obj;
+    a.n_charuco = h->n_charuco;
+    a.ch_boards = h->d_ch_boards;
+    a.ch_keys = h->d_ch_keys;
+    a.ch_marker = h->d_ch_marker;
+    a.ch_obj = h->d_ch_obj;
+    a.has_cam = cam ? 1 : 0;
+    a.cam = make_camera(cam);
+    a.n_rej = d_count + 1;
+    a.rej = d_rej;
+    a.max_rej = FID_MAX_REJECTED;
+    a.max_markers = max_markers;
+    a.count = d_count;
+    a.ids = d_ids;
+    a.corners = d_corners;
+    a.n_rec = d_count + 2;
+    a.rec_idx = d_rec_idx;
+    a.rec_board = d_rec_board;
+    a.overflow = reinterpret_cast<uint32_t*>(d_count + 3);
+    k_marker_refine<<<1, MREFINE_THREADS, MREFINE_SMEM, h->stream>>>(a);
+    CK(cudaGetLastError());
+    int32_t out[4];
+    CK(cudaMemcpyAsync(out, d_count, sizeof(out), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (out[3]) return FID_ERR_CAPACITY;
+    const int nr = out[2];
+    if (nr > 0) {
+        CK(cudaMemcpy(ids + n, d_ids + n, sizeof(int32_t) * nr, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(corners + (size_t)8 * n, d_corners + (size_t)8 * n, sizeof(float) * 8 * nr, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(recovered_idx, d_rec_idx, sizeof(int32_t) * nr, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(recovered_board, d_rec_board, sizeof(int32_t) * nr, cudaMemcpyDeviceToHost));
+    }
+    *n_out = out[0];
     return FID_OK;
 }
 

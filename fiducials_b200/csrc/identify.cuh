@@ -153,19 +153,27 @@ struct IdentifyResult {
     int rotation;  // number of corner rotations to apply
 };
 
+// The cell bits of a quad (_extractBits): cell c = y*cells + x is bit c of lo for c < 64, bit c-64 of hi otherwise (7x7 markers
+// have 81 cells).
+struct CellBits {
+    unsigned long long lo, hi;
+    bool ok;  // false: the quad gives no perspective transform
+    FID_HD int at(int c) const { return (int)(((c < 64 ? lo >> c : hi >> (c - 64))) & 1ull); }
+};
+
+// _extractBits: perspective removal (nearest warp), Otsu or the minOtsuStdDev rule, cell votes.  ok = false where the quad
+// gives no perspective transform.  Returned by value: through an out pointer k_identify_first spilled more.
 // `img` : S*S bytes of scratch, `hist`: 256 ints of scratch (zeroed by this function).
-// dict  : n_markers x 4 rotations packed as little-endian byte strings in 64-bit words.
 template <class Lanes, class Img>
-FID_HD IdentifyResult identify_candidate(const Lanes& L, const Img& gray, int W, int H, const QuadF& quad, const DevParams& P, const unsigned long long* dict, uint8_t* img,
-                                         int* hist) {
-    IdentifyResult res = {-1, 0};
+FID_HD CellBits extract_bits(const Lanes& L, const Img& gray, int W, int H, const QuadF& quad, const DevParams& P, uint8_t* img, int* hist) {
+    CellBits out = {0ull, 0ull, false};
     const int cells = P.marker_size + 2 * P.marker_border_bits;
     const int cell = P.px_per_cell;
     const int S = cells * cell;
     const int margin = (int)(P.ignored_margin_per_cell * cell);
     double M[9], Mi[9];
-    if (!perspective_transform(quad, (double)(S - 1), M)) return res;
-    if (!invert3x3(M, Mi)) return res;
+    if (!perspective_transform(quad, (double)(S - 1), M)) return out;
+    if (!invert3x3(M, Mi)) return out;
     for (int i = L.lane(); i < 256; i += L.count()) hist[i] = 0;
     L.sync();
     const int half = cell / 2;
@@ -190,7 +198,6 @@ FID_HD IdentifyResult identify_candidate(const Lanes& L, const Img& gray, int W,
     double var = (double)s2 * scale - mean * mean;
     var = var > 0.0 ? var : 0.0;
     const double stddev = sqrt(var);
-    // cell c = y*cells + x: bit c of bits_lo for c < 64, bit c-64 of bits_hi otherwise (7x7 markers have 81 cells)
     unsigned long long bits_lo = 0, bits_hi = 0;
     if (stddev < P.min_otsu_stddev) {
         if (mean > 127.0) bits_lo = bits_hi = ~0ull;  // all white (bits beyond cells*cells are never read)
@@ -213,36 +220,55 @@ FID_HD IdentifyResult identify_candidate(const Lanes& L, const Img& gray, int W,
         bits_lo = L.or_u64(mine);
         bits_hi = cells * cells > 64 ? L.or_u64(mine_hi) : 0ull;
     }
-    auto cell_bit = [&](int c) -> int { return (int)(((c < 64 ? bits_lo >> c : bits_hi >> (c - 64))) & 1ull); };
+    out.lo = bits_lo;
+    out.hi = bits_hi;
+    out.ok = true;
+    return out;
+}
+
+// The inner bits as a byte list (getByteListFromBits: row-major, MSB first, last partial byte right aligned) packed into a u64 the
+// way the dictionary words are.
+FID_HD unsigned long long inner_code(const CellBits& b, const DevParams& P) {
+    const int cells = P.marker_size + 2 * P.marker_border_bits;
+    const int bb = P.marker_border_bits, ms = P.marker_size;
+    unsigned long long cand = 0;
+    int k = 0, cur = 0, nbits = 0, byte_i = 0;
+    const int total = ms * ms;
+    for (int y = 0; y < ms; y++)
+        for (int x = 0; x < ms; x++) {
+            cur = (cur << 1) | b.at((y + bb) * cells + x + bb);
+            nbits++;
+            k++;
+            if (nbits == 8 || k == total) {
+                cand |= (unsigned long long)cur << (8 * byte_i);
+                byte_i++;
+                cur = 0;
+                nbits = 0;
+            }
+        }
+    return cand;
+}
+
+// `img` : S*S bytes of scratch, `hist`: 256 ints of scratch (zeroed by this function).
+// dict  : n_markers x 4 rotations packed as little-endian byte strings in 64-bit words.
+template <class Lanes, class Img>
+FID_HD IdentifyResult identify_candidate(const Lanes& L, const Img& gray, int W, int H, const QuadF& quad, const DevParams& P, const unsigned long long* dict, uint8_t* img,
+                                         int* hist) {
+    IdentifyResult res = {-1, 0};
+    const CellBits bits = extract_bits(L, gray, W, H, quad, P, img, hist);
+    if (!bits.ok) return res;
     // border errors (_getBorderErrors) -- number of white bits in the border ring
+    const int cells = P.marker_size + 2 * P.marker_border_bits;
     const int bb = P.marker_border_bits, ms = P.marker_size;
     int border_errors = 0;
     for (int y = 0; y < cells; y++)
         for (int x = 0; x < cells; x++) {
             const bool in_border = y < bb || y >= cells - bb || x < bb || x >= cells - bb;
-            if (in_border && cell_bit(y * cells + x)) border_errors++;
+            if (in_border && bits.at(y * cells + x)) border_errors++;
         }
     const int max_border = (int)((double)(ms * ms) * P.max_err_border_rate);
     if (border_errors > max_border) return res;
-    // inner bits -> byte list (row-major, MSB first, last partial byte right aligned) -> u64
-    unsigned long long cand = 0;
-    {
-        int k = 0, cur = 0, nbits = 0, byte_i = 0;
-        const int total = ms * ms;
-        for (int y = 0; y < ms; y++)
-            for (int x = 0; x < ms; x++) {
-                const int b = cell_bit((y + bb) * cells + x + bb);
-                cur = (cur << 1) | b;
-                nbits++;
-                k++;
-                if (nbits == 8 || k == total) {
-                    cand |= (unsigned long long)cur << (8 * byte_i);
-                    byte_i++;
-                    cur = 0;
-                    nbits = 0;
-                }
-            }
-    }
+    const unsigned long long cand = inner_code(bits, P);
     const int max_corr = (int)((double)P.max_correction_bits * P.error_correction_rate);
     int first = 0x7fffffff;
     for (int m = L.lane(); m < P.n_markers; m += L.count()) {

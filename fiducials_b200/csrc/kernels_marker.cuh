@@ -9,6 +9,7 @@
 //   k_board_pose  opt-in, after k_finish (and k_pose_hypotheses): one warp per (frame, board), one solvePnP over every
 //                 detected marker of the board (board_pnp.cuh)
 //   k_charuco     opt-in, last: one block per (frame, ChArUco board), its chessboard corners and pose (charuco.cuh)
+//   k_marker_refine  one block per frame: board markers recovered from the rejected candidates (marker_refine.cuh)
 #pragma once
 #include <cuda_runtime.h>
 
@@ -19,6 +20,7 @@
 #include "contour_refine.cuh"
 #include "identify.cuh"
 #include "ippe.cuh"
+#include "marker_refine.cuh"
 #include "pnp.cuh"
 #include "quad_group.cuh"
 #include "subpix.cuh"
@@ -1081,6 +1083,247 @@ __global__ void __launch_bounds__(CHARUCO_THREADS) k_charuco(const CharucoArgs a
             charuco_pack(po, status, &r);
             a.out[(size_t)f * a.n_boards + b] = r;
         }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Recovery of missed board markers (marker_refine.cuh): the marker boards, then the ChArUco boards, one refineDetectedMarkers call
+// after another, each on the lists the previous one left.
+struct MarkerRefineArgs {
+    const uint8_t* src;
+    size_t row_stride, frame_stride;
+    int enc, W, H;
+    DevParams P;
+    const unsigned long long* dict;  // n_markers x 4 words
+    const float* subpix_masks;       // windows 1..5 (k_finish's table)
+    MarkerRefineParams rp;
+    int n_boards;                    // marker boards, tables as BoardPoseArgs
+    const int32_t *board_off, *board_keys, *board_marker;
+    const float* board_obj;
+    int n_charuco;                   // ChArUco boards, tables as CharucoArgs
+    const CharucoBoardDev* ch_boards;
+    const int32_t *ch_keys, *ch_marker;
+    const float* ch_obj;
+    int has_cam;
+    Camera cam;
+    const int32_t* n_rej;            // [F]
+    const float* rej;                // [F][max_rej][8]
+    int max_rej, max_markers;
+    int32_t* count;                  // [F]                    the detections; recovered markers are appended
+    int32_t* ids;                    // [F][max_markers]
+    float* corners;                  // [F][max_markers][8]
+    int32_t* n_rec;                  // [F]
+    int32_t* rec_idx;                // [F][max_markers]       index into the frame's rejected list
+    int32_t* rec_board;              // [F][max_markers]       marker board b, or FID_MAX_BOARDS + ChArUco board c
+    uint32_t* overflow;              // bit 32: a recovered marker found no slot below max_markers; refinement of the frame stops there
+};
+
+#define MREFINE_THREADS 128
+#define FID_MAX_BOARD_ROWS 4096
+// dynamic shared memory: the matched points of solvePnP (normalised, object, image), board ids in board order, detected-row bits,
+// the rejected candidates taken, and one warp's bit-extraction scratch
+#define MREFINE_SMEM (4 * FID_MAX_MARKERS * (2 * 8 + 3 * 4 + 2 * 4) + FID_MAX_BOARD_ROWS * 4 + FID_MAX_BOARD_ROWS / 8 + FID_MAX_REJECTED + 256 * 4 + FID_MAX_WARP_SIDE_SQ)
+
+// One block per frame.  Per board: threads find the detected board rows, warp 0 solves the pose (or the homography), then chunks of
+// board rows are projected and screened by the threads, compacted in board order, and warp 0 replays the greedy matching over the
+// survivors with warp-cooperative bit extraction.
+__global__ void __launch_bounds__(MREFINE_THREADS) k_marker_refine(const MarkerRefineArgs a) {
+    extern __shared__ __align__(16) unsigned char mrefine_smem[];
+    double* s_mn = (double*)mrefine_smem;
+    float* s_obj = (float*)(s_mn + 2 * 4 * FID_MAX_MARKERS);
+    float* s_img = s_obj + 3 * 4 * FID_MAX_MARKERS;
+    int32_t* s_rowid = (int32_t*)(s_img + 2 * 4 * FID_MAX_MARKERS);
+    uint32_t* s_found = (uint32_t*)(s_rowid + FID_MAX_BOARD_ROWS);
+    int* s_hist = (int*)(s_found + FID_MAX_BOARD_ROWS / 32);
+    uint8_t* s_taken = (uint8_t*)(s_hist + 256);
+    uint8_t* s_warp = s_taken + FID_MAX_REJECTED;
+    __shared__ int32_t s_detrow[FID_MAX_MARKERS], s_first[FID_MAX_MARKERS], s_hrow[FID_MAX_MARKERS], s_hdet[FID_MAX_MARKERS];
+    __shared__ int32_t s_surv[MREFINE_THREADS];
+    __shared__ float s_proj[MREFINE_THREADS][8];
+    __shared__ double s_p[9];
+    __shared__ int s_n, s_nrec, s_ntaken, s_ok, s_m, s_ns, s_full, s_wcnt[MREFINE_THREADS / 32];
+    const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int n_rej = min(a.n_rej[f], min(a.max_rej, FID_MAX_REJECTED));
+    const float* rej = a.rej + (size_t)f * a.max_rej * 8;
+    int32_t* ids = a.ids + (size_t)f * a.max_markers;
+    float* corners = a.corners + (size_t)f * a.max_markers * 8;
+    const FrameImg gray{a.src + (size_t)f * a.frame_stride, a.row_stride, a.enc};
+    for (int j = tid; j < n_rej; j += MREFINE_THREADS) s_taken[j] = 0;
+    if (tid == 0) {
+        s_n = min(a.count[f], min(a.max_markers, FID_MAX_MARKERS));
+        s_nrec = 0;
+        s_ntaken = 0;
+        s_full = 0;
+    }
+    for (int bi = 0; bi < a.n_boards + a.n_charuco; bi++) {
+        __syncthreads();
+        if (s_full) break;
+        const int n0 = s_n;
+        if (n0 == 0 || s_ntaken == n_rej) continue;  // refineDetectedMarkers returns at once
+        RefineBoardView B;
+        int label;
+        if (bi < a.n_boards) {
+            const int off = a.board_off[bi];
+            B = RefineBoardView{a.board_off[bi + 1] - off, a.board_keys + off, a.board_marker + off, a.board_obj + (size_t)off * 12};
+            label = bi;
+        } else {
+            const CharucoBoardDev bd = a.ch_boards[bi - a.n_boards];
+            B = RefineBoardView{bd.n_markers, a.ch_keys + bd.marker_off, a.ch_marker + bd.marker_off, a.ch_obj + (size_t)bd.marker_off * 12};
+            label = FID_MAX_BOARDS + bi - a.n_boards;
+        }
+        // 1. board ids in board order, the detected rows (against the detections this call starts with)
+        for (int k = tid; k < B.n; k += MREFINE_THREADS) s_rowid[B.marker_of[k]] = B.keys[k];
+        for (int w = tid; w < (B.n + 31) / 32; w += MREFINE_THREADS) s_found[w] = 0;
+        if (tid == 0) s_m = 0;
+        __syncthreads();
+        for (int j = tid; j < n0; j += MREFINE_THREADS) {
+            const int k = board_find(B.keys, B.n, ids[j]);
+            const int row = k < 0 ? -1 : B.marker_of[k];
+            s_detrow[j] = row;
+            if (row >= 0) atomicOr(&s_found[row >> 5], 1u << (row & 31));
+        }
+        __syncthreads();
+        if (!a.has_cam) {  // the homography's points: the first detection of every detected board row, in board order
+            for (int j = tid; j < n0; j += MREFINE_THREADS) {
+                const int row = s_detrow[j];
+                bool first = row >= 0;
+                for (int i = 0; i < j && first; i++) first = s_detrow[i] != row;
+                s_first[j] = first;
+            }
+            __syncthreads();
+            for (int j = tid; j < n0; j += MREFINE_THREADS) {
+                if (!s_first[j]) continue;
+                const int row = s_detrow[j];
+                int rank = 0;
+                for (int i = 0; i < n0; i++) rank += s_first[i] && s_detrow[i] < row;
+                s_hrow[rank] = row;
+                s_hdet[rank] = j;
+                atomicAdd(&s_m, 1);
+            }
+            __syncthreads();
+        }
+        // 2. the prediction: warp 0 solves the board pose or the homography
+        if (warp == 0) {
+            int ok = 0;
+            if (a.has_cam) {
+                int m = 0;
+                for (int j0 = 0; j0 < n0; j0 += 32) {
+                    const int j = j0 + lane;
+                    const int row = j < n0 ? s_detrow[j] : -1;
+                    const unsigned hit = __ballot_sync(0xffffffffu, row >= 0);
+                    if (row >= 0) {
+                        const int pos = m + __popc(hit & ((1u << lane) - 1u));
+                        for (int c = 0; c < 12; c++) s_obj[pos * 12 + c] = B.obj[(size_t)row * 12 + c];
+                        for (int c = 0; c < 8; c++) s_img[pos * 8 + c] = corners[(size_t)j * 8 + c];
+                    }
+                    m += __popc(hit);
+                }
+                __syncwarp();
+                if (m > 0) {
+                    BoardPoseOut po;
+                    solve_board_pose(4 * m, s_obj, s_img, s_mn, a.cam, &po);
+                    ok = po.status == 1;  // -1: cv2's solvePnP raises
+                    if (ok && lane == 0)
+                        for (int k = 0; k < 3; k++) {
+                            s_p[k] = po.rvec[k];
+                            s_p[3 + k] = po.tvec[k];
+                        }
+                }
+            } else {
+                bool flat = true;  // cv2 asserts that every board point has the z of the first
+                for (int i = lane; i < 4 * B.n; i += 32) flat = flat && B.obj[3 * i + 2] == B.obj[2];
+                const int m = s_m;
+                if (__all_sync(0xffffffffu, flat) && m > 0) {
+                    double Hm[9];
+                    ok = board_homography(4 * m, [&](int i, float s[2], float d[2]) {
+                        const int row = s_hrow[i >> 2], c = i & 3;
+                        s[0] = B.obj[(size_t)row * 12 + 3 * c];
+                        s[1] = B.obj[(size_t)row * 12 + 3 * c + 1];
+                        d[0] = corners[(size_t)s_hdet[i >> 2] * 8 + 2 * c];
+                        d[1] = corners[(size_t)s_hdet[i >> 2] * 8 + 2 * c + 1];
+                    }, Hm);
+                    if (ok && lane == 0)
+                        for (int k = 0; k < 9; k++) s_p[k] = Hm[k];
+                }
+            }
+            if (lane == 0) s_ok = ok;
+        }
+        __syncthreads();
+        if (!s_ok) continue;
+        double p[9], R[9];
+        for (int k = 0; k < 9; k++) p[k] = s_p[k];
+        if (a.has_cam) rodrigues_v2m(p, R, nullptr);
+        // 3. chunks of board rows: project the undetected ones, keep those with a candidate in reach, replay the matching in order
+        for (int r0 = 0; r0 < B.n; r0 += MREFINE_THREADS) {
+            const int r = r0 + tid;
+            float pr[8];
+            bool keep = r < B.n && !((s_found[r >> 5] >> (r & 31)) & 1u);
+            if (keep) {
+                if (a.has_cam) refine_project(B.obj, r, R, p, a.cam, pr);
+                else refine_transform(B.obj, r, p, pr);
+                keep = refine_has_candidate(a.rp, pr, n_rej, rej, s_taken);
+            }
+            const unsigned m = __ballot_sync(0xffffffffu, keep);
+            if (lane == 0) s_wcnt[warp] = __popc(m);
+            __syncthreads();
+            int pos = __popc(m & ((1u << lane) - 1u));
+            for (int w = 0; w < warp; w++) pos += s_wcnt[w];
+            if (keep) {
+                s_surv[pos] = r;
+                for (int c = 0; c < 8; c++) s_proj[pos][c] = pr[c];
+            }
+            if (tid == 0) {
+                int ns = 0;
+                for (int w = 0; w < MREFINE_THREADS / 32; w++) ns += s_wcnt[w];
+                s_ns = ns;
+            }
+            __syncthreads();
+            if (warp == 0) {
+                const WarpLanes L;
+                for (int s = 0; s < s_ns; s++) {
+                    const int id = s_rowid[s_surv[s]];
+                    float q[8];
+                    const int j = refine_match(L, gray, a.W, a.H, a.P, a.dict, a.rp, id, s_proj[s], n_rej, rej, s_taken, s_warp, s_hist, q);
+                    if (j < 0) continue;
+                    const int n = s_n;
+                    if (n >= a.max_markers || n >= FID_MAX_MARKERS) {
+                        // no slot for a marker cv2 would append: stop refining this frame.  Going on without it would let later
+                        // markers take the candidate this one took in cv2, and every result after it would differ from cv2's.
+                        if (lane == 0) {
+                            atomicOr(a.overflow, 32u);
+                            s_full = 1;
+                        }
+                        break;
+                    }
+                    if (lane < 4) {
+                        float xy[2] = {q[2 * lane], q[2 * lane + 1]};
+                        if (a.P.corner_refine == 1) {
+                            float patch[(2 * FID_SUBPIX_MAX_WIN + 3) * (2 * FID_SUBPIX_MAX_WIN + 3)];
+                            refine_subpix_corner(gray, a.W, a.H, a.P, a.subpix_masks, q, lane, xy, patch);
+                        }
+                        corners[(size_t)n * 8 + 2 * lane] = xy[0];
+                        corners[(size_t)n * 8 + 2 * lane + 1] = xy[1];
+                    }
+                    if (lane == 0) {
+                        ids[n] = id;
+                        s_taken[j] = 1;
+                        a.rec_idx[(size_t)f * a.max_markers + s_nrec] = j;
+                        a.rec_board[(size_t)f * a.max_markers + s_nrec] = label;
+                        s_nrec++;
+                        s_ntaken++;
+                        s_n = n + 1;
+                    }
+                    __syncwarp();
+                }
+            }
+            __syncthreads();
+            if (s_full) break;
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        a.count[f] = s_n;
+        a.n_rec[f] = s_nrec;
     }
 }
 

@@ -266,6 +266,38 @@ class Detector:
                                              cxy.ctypes.data_as(C.c_void_p)), "fid_last_charuco")
         return [self._charuco_split([recs[f * nb.value + b] for b in range(nb.value)], cids[f], cxy[f]) for f in range(nf.value)]
 
+    def set_marker_refinement(self, min_rep_distance=10.0, error_correction_rate=3.0, check_all_orders=True):
+        """fid_set_marker_refinement: cv::aruco::RefineParameters for refine_markers (min_rep_distance=None turns it off)."""
+        p = _lib.fid_marker_refine_params()
+        if min_rep_distance is not None:
+            p.enable, p.min_rep_distance, p.error_correction_rate, p.check_all_orders = 1, min_rep_distance, error_correction_rate, int(bool(check_all_orders))
+        _lib.check(self.lib.fid_set_marker_refinement(self.h, C.byref(p)), "fid_set_marker_refinement")
+
+    def refine_markers(self, frame, ids, corners, rejected, K=None, D=None):
+        """fid_refine_detected_markers: cv2.aruco.ArucoDetector.refineDetectedMarkers against every marker board and then every
+        ChArUco board set, for one frame and the lists of its detection (ids [n], corners [n, 4, 2], rejected [m, 4, 2]).  Returns
+        what cv2 returns: ids, corners, the rejected candidates left, and recovered_idx (indices into `rejected`), plus the board of
+        each recovered marker (b for marker board b, FID_MAX_BOARDS + c for ChArUco board c)."""
+        frame = np.ascontiguousarray(frame, np.uint8)
+        H, W = frame.shape[:2]
+        ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+        n = len(ids)
+        oi = np.zeros(MAXM, np.int32)
+        oc = np.zeros((MAXM, 8), np.float32)
+        oi[:n] = ids
+        oc[:n] = np.asarray(corners, np.float32).reshape(-1, 8)
+        rej = np.ascontiguousarray(np.asarray(rejected, np.float32).reshape(-1, 8))
+        ri, rb = np.zeros(MAXM, np.int32), np.zeros(MAXM, np.int32)
+        nout = C.c_int(0)
+        cam = None if K is None else C.byref(_camera(K, D))
+        _lib.check(self.lib.fid_refine_detected_markers(self.h, frame.ctypes.data_as(C.c_void_p), W, H, frame.strides[0], n, oi.ctypes.data_as(C.c_void_p),
+                                                        oc.ctypes.data_as(C.c_void_p), MAXM, len(rej), rej.ctypes.data_as(C.c_void_p), cam, C.byref(nout),
+                                                        ri.ctypes.data_as(C.c_void_p), rb.ctypes.data_as(C.c_void_p)), "fid_refine_detected_markers")
+        nr = nout.value - n
+        taken = set(ri[:nr].tolist())
+        left = np.array([r for k, r in enumerate(rej) if k not in taken], np.float32).reshape(-1, 4, 2)
+        return oi[: nout.value].copy(), oc[: nout.value].reshape(-1, 4, 2).copy(), left, ri[:nr].copy(), rb[:nr].copy()
+
     def debug_threshold(self, bgr):
         bgr = np.ascontiguousarray(bgr, np.uint8)
         H, W = bgr.shape[:2]

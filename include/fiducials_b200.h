@@ -253,6 +253,36 @@ int fid_detect_charuco(fid_detector* h, const uint8_t* bgr, int width, int heigh
 int fid_last_charuco(fid_detector* h, int max_slots, int* n_frames, int* n_boards, int* n_slots, fid_charuco_result* results, int32_t* corner_ids,
                      float* corner_xy);
 
+/* Recovery of missed board markers (NEW), as cv::aruco::ArucoDetector::refineDetectedMarkers(image, board, detectedCorners,
+ * detectedIds, rejectedCorners, K, D, recoveredIdxs) of OpenCV 4.13 computes it with RefineParameters(min_rep_distance,
+ * error_correction_rate, check_all_orders).  The board predicts where each of its markers that was not detected should be (with a
+ * camera through solvePnP over the detected board markers and projectPoints; without one through a homography, for boards whose points
+ * share one z); the first rejected candidate, in list order, whose corners all lie within min_rep_distance of the prediction and whose
+ * inner bits differ from the marker's code in fewer than int(max correction bits * error_correction_rate) bits (no bit check when
+ * error_correction_rate < 0) becomes that marker, with cornerSubPix under CORNER_REFINE_SUBPIX.  Every marker board set with
+ * fid_set_boards, then every ChArUco board set with fid_set_charuco_boards, is one such call on the lists the previous call left. */
+#define FID_MAX_REJECTED 4096
+typedef struct fid_marker_refine_params {
+    int32_t enable;                /* 0 = off (the default) */
+    float min_rep_distance;        /* px, > 0 (cv2 default 10) */
+    float error_correction_rate;   /* cv2 default 3; < 0 = no bit check; 0 recovers nothing (the bit test is strict) */
+    int32_t check_all_orders;      /* try the 4 corner orders of a candidate (cv2 default 1) */
+} fid_marker_refine_params;
+/* Set the refinement parameters (copied).  The batch calls do not refine in this version; the setting is what
+ * fid_refine_detected_markers uses.  FID_ERR_INVALID_ARG for min_rep_distance <= 0 or non-finite values, or while batches are in
+ * flight. */
+int fid_set_marker_refinement(fid_detector* h, const fid_marker_refine_params* params);
+/* refineDetectedMarkers for one frame (in the fid_set_input_encoding format) and lists the caller already has, against every board
+ * set: ids / corners hold n detections ([.][4][2] floats) and receive the recovered markers after them (capacity max_markers <=
+ * FID_MAX_MARKERS); rejected [n_rejected][4][2] (n_rejected <= FID_MAX_REJECTED) is detectMarkers' rejectedImgPoints.  cam may be
+ * NULL.  *n_out = the number of detections after; recovered_idx / recovered_board [max_markers]: per recovered marker, in recovery
+ * order, its index into rejected as passed in and its board (b for marker board b, FID_MAX_BOARDS + c for ChArUco board c).
+ * FID_ERR_INVALID_ARG if refinement is off, no board is set or while batches are in flight; FID_ERR_CAPACITY, with nothing written,
+ * if the recovered markers do not fit in max_markers. */
+int fid_refine_detected_markers(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int n, int32_t* ids, float* corners,
+                                int max_markers, int n_rejected, const float* rejected, const fid_camera* cam, int* n_out, int32_t* recovered_idx,
+                                int32_t* recovered_board);
+
 /* Pixel format of the frames handed to every entry point that takes `bgr` (default FID_ENC_BGR8).  The
  * reference converts whatever the camera publishes with cv_bridge::toCvCopy(msg, BGR8)
  * (aruco_detect.cpp:348) before detectMarkers turns it into gray again; the library takes the camera's own
