@@ -62,6 +62,12 @@ struct Slot {
     fid_charuco_result* d_out_ch = nullptr;            // fid_set_charuco_boards: [max_batch][FID_MAX_CHARUCO_BOARDS]
     int32_t* d_out_ch_ids = nullptr;                   // [max_batch][ch_slot_cap]
     float* d_out_ch_xy = nullptr;                      // [max_batch][ch_slot_cap][2]
+    // fid_set_batch_marker_refinement: allocated by the first enable
+    int32_t* d_rej_n = nullptr;                        // [max_batch]                 k_rejected
+    float* d_rej = nullptr;                            // [max_batch][max_sel][8]
+    int32_t* d_mr_nrec = nullptr;                      // [max_batch]                 k_marker_refine
+    int32_t* d_mr_idx = nullptr;                       // [max_batch][max_markers]
+    int32_t* d_mr_board = nullptr;                     // [max_batch][max_markers]
     // pinned host mirrors
     int32_t* h_out_count = nullptr;
     int32_t* h_out_ids = nullptr;
@@ -73,6 +79,11 @@ struct Slot {
     int32_t* h_out_ch_ids = nullptr;
     float* h_out_ch_xy = nullptr;
     int ch_slot_cap = 0;
+    int32_t* h_rej_n = nullptr;
+    float* h_rej = nullptr;
+    int32_t* h_mr_nrec = nullptr;
+    int32_t* h_mr_idx = nullptr;
+    int32_t* h_mr_board = nullptr;
     Counters* h_counters = nullptr;
     int* h_nsel = nullptr;
     int* h_nrawc = nullptr;
@@ -102,7 +113,7 @@ struct fid_detector {
     struct Pending {
         int first_slot, n_chunks, n_frames, w, h;
         int64_t launches;
-        bool pose, hyp, board, charuco;
+        bool pose, hyp, board, charuco, refine;
     } pending[MAX_SLOTS]{};
     int pend_head = 0, pend_count = 0, slots_in_use = 0, slot_next = 0;
     cudaStream_t slot_stream[MAX_SLOTS] = {};
@@ -164,11 +175,20 @@ struct fid_detector {
     fid_marker_refine_params mrefine{};              // enable = 0: off
     int32_t* d_mr_i = nullptr;                       // count, n_rejected, n_recovered, overflow, ids, recovered idx, recovered board
     float* d_mr_f = nullptr;                         // corners [FID_MAX_MARKERS][8], rejected [FID_MAX_REJECTED][8]
+    int batch_refine = 0;                            // fid_set_batch_marker_refinement
+    bool last_mr_valid = false;                      // the batch last returned refined (fid_last_marker_refinement)
+    int last_mr_frames = 0;
+    std::vector<int32_t> last_mr_nrec, last_mr_nrej;  // [last_mr_frames]
+    std::vector<int32_t> last_mr_idx, last_mr_board;  // frame after frame, last_mr_nrec[f] each
+    std::vector<float> last_mr_rej;                   // frame after frame, last_mr_nrej[f] x 8 each
+    int32_t* d_dbg_rej_n = nullptr;                  // fid_debug_rejected: count, then [max_sel][8] floats
+    float* d_dbg_rej = nullptr;
     float stage_ms[ST_COUNT + N_WALK_ROUNDS]{};
     int64_t counters[8]{};
     cudaEvent_t t0 = nullptr, t1 = nullptr;
     // last geometry (for debug calls)
     int last_w = 0, last_h = 0, last_frames = 0;
+    bool detected = false;  // fid_detect has run: slot 0 holds a frame's candidates (fid_debug_rejected)
 };
 
 static const char* kErr[] = {"ok", "invalid argument", "no usable CUDA device (this library has no CPU fallback)", "CUDA runtime error", "unsupported parameter or dictionary",
@@ -348,10 +368,12 @@ static void free_slot(Slot& s) {
                      s.d_raw,         s.d_nraw,          s.fs.quads_tmp,    s.fs.per_tmp,     s.fs.quads,       s.fs.per,         s.fs.close_bits, s.fs.group_id,
                      s.fs.group_members, s.fs.next_in_group, s.fs.group_head, s.fs.group_tail, s.fs.close_count, s.fs.close_idx,   s.fs.close_off,  s.fs.selected,
                      s.fs.sel_idx,    s.d_nsel,          s.d_nrawc,         s.d_cand_id,      s.d_cand_corners, s.d_out_count,    s.d_out_ids,     s.d_out_corners,
-                     s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp, s.d_out_board, s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy};
+                     s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp, s.d_out_board, s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy,
+                     s.d_rej_n,       s.d_rej,           s.d_mr_nrec,       s.d_mr_idx,       s.d_mr_board};
     for (void* p : dptrs)
         if (p) cudaFree(p);
-    void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp, s.h_out_board, s.h_out_ch, s.h_out_ch_ids, s.h_out_ch_xy};
+    void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp, s.h_out_board, s.h_out_ch, s.h_out_ch_ids, s.h_out_ch_xy,
+                     s.h_rej_n,     s.h_rej,     s.h_mr_nrec,    s.h_mr_idx,   s.h_mr_board};
     for (void* p : hptrs)
         if (p) cudaFreeHost(p);
     for (int i = 0; i <= ST_COUNT; i++)
@@ -504,7 +526,7 @@ extern "C" int fid_destroy(fid_detector* h) {
     void* ptrs[] = {h->d_prune, h->d_dict, h->d_pf[0], h->d_pf[1], h->d_lut_prev, h->d_lut_next, h->d_subpix_masks, h->d_override_ids, h->d_override_lens, h->d_pose_ids, h->d_pose_corners, h->d_pose_out, h->d_hyp_list,
                      h->d_board_off, h->d_board_keys, h->d_board_marker, h->d_board_obj, h->d_board_count, h->d_board_list, h->d_ch_boards, h->d_ch_keys,
                      h->d_ch_marker, h->d_ch_ids, h->d_ch_near_n, h->d_ch_near_idx, h->d_ch_near_corner, h->d_ch_obj, h->d_ch_chess, h->d_ch_masks,
-                     h->d_ch_count, h->d_ch_list, h->d_ch_list_ids, h->d_ch_list_xy, h->d_mr_i, h->d_mr_f};
+                     h->d_ch_count, h->d_ch_list, h->d_ch_list_ids, h->d_ch_list_xy, h->d_mr_i, h->d_mr_f, h->d_dbg_rej_n, h->d_dbg_rej};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     for (int i = 0; i < 2; i++)
@@ -633,8 +655,39 @@ static CharucoArgs charuco_args(const fid_detector* h, const uint8_t* src, size_
     return a;
 }
 
+// k_marker_refine's frames, parameters and boards; the caller sets the lists.
+static MarkerRefineArgs marker_refine_args(const fid_detector* h, const uint8_t* src, size_t row_stride, size_t frame_stride, int W, int H, const fid_camera* cam) {
+    MarkerRefineArgs a{};
+    a.src = src;
+    a.row_stride = row_stride;
+    a.frame_stride = frame_stride;
+    a.enc = h->enc;
+    a.W = W;
+    a.H = H;
+    a.P = h->P;
+    a.dict = h->d_dict;
+    a.subpix_masks = h->d_subpix_masks;
+    a.rp = MarkerRefineParams{h->mrefine.min_rep_distance, h->mrefine.error_correction_rate, h->mrefine.check_all_orders ? 1 : 0};
+    a.n_boards = h->n_boards;
+    a.board_off = h->d_board_off;
+    a.board_keys = h->d_board_keys;
+    a.board_marker = h->d_board_marker;
+    a.board_obj = h->d_board_obj;
+    a.n_charuco = h->n_charuco;
+    a.ch_boards = h->d_ch_boards;
+    a.ch_keys = h->d_ch_keys;
+    a.ch_marker = h->d_ch_marker;
+    a.ch_obj = h->d_ch_obj;
+    a.has_cam = cam ? 1 : 0;
+    a.cam = make_camera(cam);
+    return a;
+}
+
+// A batch refines only with the batch switch, the refinement parameters and a board to refine against.
+static bool batch_refines(const fid_detector* h) { return h->batch_refine && h->mrefine.enable && h->n_boards + h->n_charuco > 0; }
+
 static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, const FrameGeom& g, const uint8_t* d_bgr, const fid_camera* cam, double fiducial_len,
-                            int n_override, int stop_after /* -1 = all */, const Slot* prev = nullptr) {
+                            int n_override, int stop_after /* -1 = all */, const Slot* prev = nullptr, bool refine = false) {
     const DevParams& P = h->P;
     const int W = g.W, H = g.H;
     int launches = 0;
@@ -909,6 +962,47 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         launch_prio(k_finish, dim3(nf), dim3(FINISH_THREADS), 0, st, 5, a);
         launches++;
     }
+    if (refine) {  // opt-in: recover missed board markers before the stages that read the markers (fid_set_batch_marker_refinement)
+        RejectedArgs ra{};
+        ra.n_sel = s.d_nsel;
+        ra.cand_id = s.d_cand_id;
+        ra.fs = s.fs;
+        ra.max_raw = h->max_raw;
+        ra.max_sel = h->max_sel;
+        ra.n_rej = s.d_rej_n;
+        ra.rej = s.d_rej;
+        launch_prio(k_rejected, dim3(nf), dim3(FINISH_THREADS), 0, st, 5, ra);
+        MarkerRefineArgs a = marker_refine_args(h, d_bgr, g.bgr_row_stride, g.bgr_frame_stride, W, H, cam);
+        a.n_rej = s.d_rej_n;
+        a.rej = s.d_rej;
+        a.max_rej = h->max_sel;
+        a.max_markers = h->max_markers;
+        a.count = s.d_out_count;
+        a.ids = s.d_out_ids;
+        a.corners = s.d_out_corners;
+        a.n_rec = s.d_mr_nrec;
+        a.rec_idx = s.d_mr_idx;
+        a.rec_board = s.d_mr_board;
+        a.overflow = &s.d_counters->overflow;
+        launch_prio(k_marker_refine, dim3(nf), dim3(MREFINE_THREADS), MREFINE_SMEM, st, 5, a);
+        launches += 2;
+        if (cam) {
+            RecoveredPoseArgs pa{};
+            pa.count = s.d_out_count;
+            pa.n_rec = s.d_mr_nrec;
+            pa.ids = s.d_out_ids;
+            pa.corners = s.d_out_corners;
+            pa.max_markers = h->max_markers;
+            pa.cam = make_camera(cam);
+            pa.fiducial_len = fiducial_len;
+            pa.n_override = n_override;
+            pa.override_ids = h->d_override_ids;
+            pa.override_lens = h->d_override_lens;
+            pa.out_tf = s.d_out_tf;
+            launch_prio(k_recovered_pose, dim3(nf), dim3(32), 0, st, 5, pa);
+            launches++;
+        }
+    }
     if (h->pose_hyp && cam) {  // opt-in: both planar hypotheses of every marker k_finish wrote (fid_set_pose_hypotheses)
         PoseHypArgs a{};
         a.nf = nf;
@@ -942,8 +1036,12 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
     return FID_OK;
 }
 
-static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose, bool with_hyp, bool with_board, bool with_charuco) {
+static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose, bool with_hyp, bool with_board, bool with_charuco, bool with_refine) {
     const size_t M = (size_t)nf * h->max_markers;
+    if (with_refine) {  // counts only: collect copies the lists at their lengths
+        CK(cudaMemcpyAsync(s.h_rej_n, s.d_rej_n, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(s.h_mr_nrec, s.d_mr_nrec, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));
+    }
     CK(cudaMemcpyAsync(s.h_out_count, s.d_out_count, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_out_ids, s.d_out_ids, sizeof(int32_t) * M, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(s.h_out_corners, s.d_out_corners, sizeof(float) * 8 * M, cudaMemcpyDeviceToHost, st));
@@ -964,9 +1062,32 @@ static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool w
 }
 
 static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* tfs, bool first_chunk,
-                   struct fid_pose_hypotheses* hyps = nullptr, fid_board_pose* boards = nullptr, int ch_first = -1) {
+                   struct fid_pose_hypotheses* hyps = nullptr, fid_board_pose* boards = nullptr, int ch_first = -1, bool refined = false) {
     CK(cudaEventSynchronize(s.done));
     int status = FID_OK;
+    if (refined) {  // the rejected lists and the recovered markers (fid_last_marker_refinement), each row at the longest frame's length
+        const cudaStream_t st = h->slot_stream[&s - h->slot];
+        int max_rej = 0, max_rec = 0;
+        for (int f = 0; f < nf; f++) {
+            max_rej = std::max(max_rej, (int)s.h_rej_n[f]);
+            max_rec = std::max(max_rec, (int)s.h_mr_nrec[f]);
+        }
+        if (max_rej)
+            CK(cudaMemcpy2DAsync(s.h_rej, sizeof(float) * 8 * max_rej, s.d_rej, sizeof(float) * 8 * h->max_sel, sizeof(float) * 8 * max_rej, nf, cudaMemcpyDeviceToHost, st));
+        if (max_rec) {
+            CK(cudaMemcpy2DAsync(s.h_mr_idx, sizeof(int32_t) * max_rec, s.d_mr_idx, sizeof(int32_t) * h->max_markers, sizeof(int32_t) * max_rec, nf, cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpy2DAsync(s.h_mr_board, sizeof(int32_t) * max_rec, s.d_mr_board, sizeof(int32_t) * h->max_markers, sizeof(int32_t) * max_rec, nf, cudaMemcpyDeviceToHost, st));
+        }
+        CK(cudaStreamSynchronize(st));
+        for (int f = 0; f < nf; f++) {
+            const int nj = s.h_rej_n[f], nr = s.h_mr_nrec[f];
+            h->last_mr_nrej.push_back(nj);
+            h->last_mr_nrec.push_back(nr);
+            h->last_mr_rej.insert(h->last_mr_rej.end(), s.h_rej + (size_t)f * max_rej * 8, s.h_rej + ((size_t)f * max_rej + nj) * 8);
+            h->last_mr_idx.insert(h->last_mr_idx.end(), s.h_mr_idx + (size_t)f * max_rec, s.h_mr_idx + (size_t)f * max_rec + nr);
+            h->last_mr_board.insert(h->last_mr_board.end(), s.h_mr_board + (size_t)f * max_rec, s.h_mr_board + (size_t)f * max_rec + nr);
+        }
+    }
     if (s.h_counters->overflow) status = FID_ERR_CAPACITY;
     for (int f = 0; f < nf; f++) {
         int n = s.h_out_count[f];
@@ -1066,9 +1187,22 @@ static void begin_last_charuco(fid_detector* h, bool ch, int n_frames) {
     h->last_ch_xy.resize((size_t)n_frames * h->charuco_slots * 2);
 }
 
-extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
-                                     const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
-                                     int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms) {
+// The same for the recovered markers and rejected lists (fid_last_marker_refinement); collect appends frame after frame.
+static void begin_last_refinement(fid_detector* h, bool refine, int n_frames) {
+    h->last_mr_valid = false;
+    if (!refine) return;
+    h->last_mr_frames = n_frames;
+    h->last_mr_nrec.clear();
+    h->last_mr_nrej.clear();
+    h->last_mr_idx.clear();
+    h->last_mr_board.clear();
+    h->last_mr_rej.clear();
+}
+
+// fid_detect_pose_batch; fid_detect (detectMarkers) passes may_refine = false.
+static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
+                             const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
+                             int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms, bool may_refine) {
     if (!h || !bgr || !counts || n_frames < 0 || width < 16 || height < 16 || width > h->max_w || height > h->max_h || max_markers < 0) return FID_ERR_INVALID_ARG;
     if (row_stride < (size_t)width * h->bpp || frame_stride < row_stride * (size_t)height) return FID_ERR_INVALID_ARG;
     if (cam && !(fiducial_len > 0)) return FID_ERR_INVALID_ARG;
@@ -1087,6 +1221,8 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
     fid_board_pose* boards = begin_last_boards(h, brd, n_frames);
     const bool chr = h->n_charuco > 0;
     begin_last_charuco(h, chr, n_frames);
+    const bool mr = may_refine && batch_refines(h);
+    begin_last_refinement(h, mr, n_frames);
     h->counters[6] = 0;
     h->stage_ms[ST_H2D] = 0;
     // software pipeline over chunks: up to n_slots chunks in flight, each on its own stream; results of
@@ -1137,9 +1273,9 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
                 h->pf_h = height;
                 h->hint_next = nullptr;
             }
-            rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, c > 0 ? &h->slot[(c - 1) % NS] : nullptr);
+            rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, c > 0 ? &h->slot[(c - 1) % NS] : nullptr, mr);
             if (rc != FID_OK) return rc;
-            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp, brd, chr);
+            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp, brd, chr, mr);
             if (rc != FID_OK) return rc;
             h->last_frames = nf;
         }
@@ -1149,14 +1285,22 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
             const int nf = std::min(B, n_frames - pc * B);
             rc = collect(h, s, nf, max_markers, counts + (size_t)pc * B, ids ? ids + (size_t)pc * B * max_markers : nullptr,
                          corners ? corners + (size_t)pc * B * max_markers * 8 : nullptr, (transforms && cam) ? transforms + (size_t)pc * B * max_markers : nullptr, pc == 0,
-                         hyps ? hyps + (size_t)pc * B * max_markers : nullptr, boards ? boards + (size_t)pc * B * h->n_boards : nullptr, chr ? pc * B : -1);
+                         hyps ? hyps + (size_t)pc * B * max_markers : nullptr, boards ? boards + (size_t)pc * B * h->n_boards : nullptr, chr ? pc * B : -1, mr);
             if (rc != FID_OK) status = rc;
         }
     }
     end_last_hypotheses(h, hyp, counts);
     h->last_board_valid = brd;
     h->last_ch_valid = chr;
+    h->last_mr_valid = mr;
     return status;
+}
+
+extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
+                                     const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
+                                     int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms) {
+    return detect_pose_batch(h, n_frames, bgr, bgr_on_device, width, height, row_stride, frame_stride, cam, fiducial_len, n_override, override_ids, override_lens,
+                             max_markers, counts, ids, corners, transforms, true);
 }
 
 extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
@@ -1176,6 +1320,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
     h->last_h = height;
     const bool contiguous = row_stride == (size_t)width * h->bpp && frame_stride == row_stride * height;
     const int first = h->slot_next;
+    const bool mr = batch_refines(h);
     h->counters[6] = 0;
     for (int c = 0; c < n_chunks; c++) {
         const int si = (first + c) % NS;
@@ -1202,9 +1347,9 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
             g = make_geom(h, width, height, (size_t)width * h->bpp, (size_t)width * h->bpp * height);
         }
         const Slot* prev = (h->slots_in_use + c) > 0 ? &h->slot[(si + NS - 1) % NS] : nullptr;
-        rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, prev);
+        rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, prev, mr);
         if (rc != FID_OK) return rc;
-        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam, h->n_boards && cam, h->n_charuco > 0);
+        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam, h->n_boards && cam, h->n_charuco > 0, mr);
         if (rc != FID_OK) return rc;
         h->last_frames = nf;
     }
@@ -1218,6 +1363,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
     pb.hyp = h->pose_hyp && cam;
     pb.board = h->n_boards && cam;
     pb.charuco = h->n_charuco > 0;
+    pb.refine = mr;
     pb.launches = h->counters[6];
     h->pend_count++;
     h->slots_in_use += n_chunks;
@@ -1236,18 +1382,20 @@ extern "C" int fid_collect_batch(fid_detector* h, int max_markers, int32_t* coun
     struct fid_pose_hypotheses* hyps = begin_last_hypotheses(h, pb.hyp, pb.n_frames, max_markers);
     fid_board_pose* boards = begin_last_boards(h, pb.board, pb.n_frames);
     begin_last_charuco(h, pb.charuco, pb.n_frames);
+    begin_last_refinement(h, pb.refine, pb.n_frames);
     for (int c = 0; c < pb.n_chunks; c++) {
         Slot& s = h->slot[(pb.first_slot + c) % NS];
         const int nf = std::min(B, pb.n_frames - c * B);
         const int rc = collect(h, s, nf, max_markers, counts + (size_t)c * B, ids ? ids + (size_t)c * B * max_markers : nullptr,
                                corners ? corners + (size_t)c * B * max_markers * 8 : nullptr, (transforms && pb.pose) ? transforms + (size_t)c * B * max_markers : nullptr, c == 0,
                                hyps ? hyps + (size_t)c * B * max_markers : nullptr, boards ? boards + (size_t)c * B * h->n_boards : nullptr,
-                               pb.charuco ? c * B : -1);
+                               pb.charuco ? c * B : -1, pb.refine);
         if (rc != FID_OK) status = rc;
     }
     end_last_hypotheses(h, pb.hyp, counts);
     h->last_board_valid = pb.board;
     h->last_ch_valid = pb.charuco;
+    h->last_mr_valid = pb.refine;
     h->pend_head = (h->pend_head + 1) % MAX_SLOTS;
     h->pend_count--;
     h->slots_in_use -= pb.n_chunks;
@@ -1257,7 +1405,8 @@ extern "C" int fid_collect_batch(fid_detector* h, int max_markers, int32_t* coun
 extern "C" int fid_detect(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int max_markers, int* n, int32_t* ids, float* corners) {
     if (!n) return FID_ERR_INVALID_ARG;
     int32_t count = 0;
-    const int rc = fid_detect_pose_batch(h, 1, bgr, 0, width, height, stride, stride * (size_t)height, nullptr, 0.0, 0, nullptr, nullptr, max_markers, &count, ids, corners, nullptr);
+    const int rc = detect_pose_batch(h, 1, bgr, 0, width, height, stride, stride * (size_t)height, nullptr, 0.0, 0, nullptr, nullptr, max_markers, &count, ids, corners, nullptr, false);
+    if (rc == FID_OK || rc == FID_ERR_CAPACITY) h->detected = true;
     *n = count;
     return rc;
 }
@@ -1605,29 +1754,7 @@ extern "C" int fid_refine_detected_markers(fid_detector* h, const uint8_t* bgr, 
         CK(cudaMemcpyAsync(d_corners, corners, sizeof(float) * 8 * n, cudaMemcpyHostToDevice, h->stream));
     }
     if (n_rejected > 0) CK(cudaMemcpyAsync(d_rej, rejected, sizeof(float) * 8 * n_rejected, cudaMemcpyHostToDevice, h->stream));
-    MarkerRefineArgs a{};
-    a.src = s.d_bgr;
-    a.row_stride = (size_t)width * h->bpp;
-    a.frame_stride = a.row_stride * height;
-    a.enc = h->enc;
-    a.W = width;
-    a.H = height;
-    a.P = h->P;
-    a.dict = h->d_dict;
-    a.subpix_masks = h->d_subpix_masks;
-    a.rp = MarkerRefineParams{h->mrefine.min_rep_distance, h->mrefine.error_correction_rate, h->mrefine.check_all_orders ? 1 : 0};
-    a.n_boards = h->n_boards;
-    a.board_off = h->d_board_off;
-    a.board_keys = h->d_board_keys;
-    a.board_marker = h->d_board_marker;
-    a.board_obj = h->d_board_obj;
-    a.n_charuco = h->n_charuco;
-    a.ch_boards = h->d_ch_boards;
-    a.ch_keys = h->d_ch_keys;
-    a.ch_marker = h->d_ch_marker;
-    a.ch_obj = h->d_ch_obj;
-    a.has_cam = cam ? 1 : 0;
-    a.cam = make_camera(cam);
+    MarkerRefineArgs a = marker_refine_args(h, s.d_bgr, (size_t)width * h->bpp, (size_t)width * h->bpp * height, width, height, cam);
     a.n_rej = d_count + 1;
     a.rej = d_rej;
     a.max_rej = FID_MAX_REJECTED;
@@ -1653,6 +1780,56 @@ extern "C" int fid_refine_detected_markers(fid_detector* h, const uint8_t* bgr, 
         CK(cudaMemcpy(recovered_board, d_rec_board, sizeof(int32_t) * nr, cudaMemcpyDeviceToHost));
     }
     *n_out = out[0];
+    return FID_OK;
+}
+
+extern "C" int fid_set_batch_marker_refinement(fid_detector* h, int enable) {
+    if (!h || h->pend_count) return FID_ERR_INVALID_ARG;
+    if (enable) {  // (a failed allocation leaves the option off; the next enable completes it)
+        CK(cudaSetDevice(h->device));
+        const size_t F = h->max_batch, M = F * h->max_markers;
+        int rc;
+#define A(expr)                  \
+    if ((rc = (expr)) != FID_OK) return rc;
+        for (int i = 0; i < h->n_slots; i++) {
+            Slot& s = h->slot[i];
+            if (!s.d_rej_n) A(dalloc(&s.d_rej_n, F));
+            if (!s.d_rej) A(dalloc(&s.d_rej, F * h->max_sel * 8));
+            if (!s.d_mr_nrec) A(dalloc(&s.d_mr_nrec, F));
+            if (!s.d_mr_idx) A(dalloc(&s.d_mr_idx, M));
+            if (!s.d_mr_board) A(dalloc(&s.d_mr_board, M));
+            if (!s.h_rej_n) A(halloc(&s.h_rej_n, F));
+            if (!s.h_rej) A(halloc(&s.h_rej, F * h->max_sel * 8));
+            if (!s.h_mr_nrec) A(halloc(&s.h_mr_nrec, F));
+            if (!s.h_mr_idx) A(halloc(&s.h_mr_idx, M));
+            if (!s.h_mr_board) A(halloc(&s.h_mr_board, M));
+        }
+#undef A
+        CK(cudaFuncSetAttribute(k_marker_refine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MREFINE_SMEM));
+    }
+    h->batch_refine = enable ? 1 : 0;
+    return FID_OK;
+}
+
+extern "C" int fid_last_marker_refinement(fid_detector* h, int max_markers, int max_rejected, int* n_frames, int32_t* n_recovered, int32_t* recovered_idx,
+                                          int32_t* recovered_board, int32_t* n_rejected, float* rejected) {
+    if (!h || max_markers < 0 || max_rejected < 0) return FID_ERR_INVALID_ARG;
+    if (!h->last_mr_valid) return FID_ERR_INVALID_ARG;
+    const int nf = h->last_mr_frames;
+    for (int f = 0; f < nf; f++)
+        if (((recovered_idx || recovered_board) && h->last_mr_nrec[f] > max_markers) || (rejected && h->last_mr_nrej[f] > max_rejected)) return FID_ERR_CAPACITY;
+    if (n_frames) *n_frames = nf;
+    size_t oi = 0, oj = 0;
+    for (int f = 0; f < nf; f++) {
+        const int nr = h->last_mr_nrec[f], nj = h->last_mr_nrej[f];
+        if (n_recovered) n_recovered[f] = nr;
+        if (n_rejected) n_rejected[f] = nj;
+        if (recovered_idx) memcpy(recovered_idx + (size_t)f * max_markers, h->last_mr_idx.data() + oi, sizeof(int32_t) * nr);
+        if (recovered_board) memcpy(recovered_board + (size_t)f * max_markers, h->last_mr_board.data() + oi, sizeof(int32_t) * nr);
+        if (rejected) memcpy(rejected + (size_t)f * max_rejected * 8, h->last_mr_rej.data() + oj * 8, sizeof(float) * 8 * nj);
+        oi += nr;
+        oj += nj;
+    }
     return FID_OK;
 }
 
@@ -1820,6 +1997,33 @@ extern "C" int fid_debug_candidates(fid_detector* h, int max_candidates, int* n,
         if (scale) scale[i] = (int)raw[i].order_hi;
         if (contour_len) contour_len[i] = raw[i].n_contour;
     }
+    return FID_OK;
+}
+
+extern "C" int fid_debug_rejected(fid_detector* h, int max_rejected, int* n, float* rejected) {
+    if (!h || !n || max_rejected < 0 || h->pend_count) return FID_ERR_INVALID_ARG;
+    if (!h->detected) return FID_ERR_INVALID_ARG;  // slot 0's candidate lists were never written
+    CK(cudaSetDevice(h->device));
+    int rc;
+    if (!h->d_dbg_rej_n && (rc = dalloc(&h->d_dbg_rej_n, 1)) != FID_OK) return rc;
+    if (!h->d_dbg_rej && (rc = dalloc(&h->d_dbg_rej, (size_t)h->max_sel * 8)) != FID_OK) return rc;
+    Slot& s = h->slot[0];
+    RejectedArgs a{};
+    a.n_sel = s.d_nsel;
+    a.cand_id = s.d_cand_id;
+    a.fs = s.fs;
+    a.max_raw = h->max_raw;
+    a.max_sel = h->max_sel;
+    a.n_rej = h->d_dbg_rej_n;
+    a.rej = h->d_dbg_rej;
+    k_rejected<<<1, FINISH_THREADS, 0, h->stream>>>(a);
+    CK(cudaGetLastError());
+    int32_t cnt = 0;
+    CK(cudaMemcpyAsync(&cnt, h->d_dbg_rej_n, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    *n = cnt;
+    if (cnt > max_rejected) return FID_ERR_CAPACITY;
+    if (cnt > 0 && rejected) CK(cudaMemcpy(rejected, h->d_dbg_rej, sizeof(float) * 8 * cnt, cudaMemcpyDeviceToHost));
     return FID_OK;
 }
 

@@ -10,11 +10,14 @@
 //                 detected marker of the board (board_pnp.cuh)
 //   k_charuco     opt-in, last: one block per (frame, ChArUco board), its chessboard corners and pose (charuco.cuh)
 //   k_marker_refine  one block per frame: board markers recovered from the rejected candidates (marker_refine.cuh)
+//   k_rejected    opt-in, after k_finish: one block per frame, detectMarkers' rejected list (candidate_tree.cuh)
+//   k_recovered_pose  opt-in, after k_marker_refine in a batch: the poses of the recovered markers
 #pragma once
 #include <cuda_runtime.h>
 
 #include "../../include/fiducials_b200.h"
 #include "board_pnp.cuh"
+#include "candidate_tree.cuh"
 #include "charuco.cuh"
 #include "common.cuh"
 #include "contour_refine.cuh"
@@ -612,7 +615,10 @@ __global__ void __launch_bounds__(FINISH_THREADS) k_finish(const FinishArgs a) {
     const int f = blockIdx.x, tid = threadIdx.x;
     const int ns = a.n_sel[f] < FID_MAX_SEL ? a.n_sel[f] : FID_MAX_SEL;
     // OpenCV 4.13 candidate hierarchy (SURVEY A.5): candidates are in descending-perimeter order; the parent of i is the
-    // nearest larger candidate whose quad contains all four corners of i
+    // nearest larger candidate whose quad contains all four corners of i.  TWIN: candidate_tree.cuh (tree_parent, tree_levels)
+    // states the same loop for k_rejected and the CPU harness; a change here must be made there too, or a candidate ends up both
+    // a marker and rejected (tests/test_gpu_batch_refine.py checks markers + rejected == selected on every frame it covers).  It
+    // stays inline here because, called through those functions, k_finish compiled to another instruction schedule.
     {
         const size_t fo = (size_t)f * a.max_raw;
         for (int i = tid; i < ns; i += FINISH_THREADS) {
@@ -718,6 +724,92 @@ __global__ void __launch_bounds__(FINISH_THREADS) k_finish(const FinishArgs a) {
             t.fiducial_area = po.area;
             a.out_tf[(size_t)f * a.max_markers + m] = t;
         }
+    }
+}
+
+// detectMarkers' rejectedImgPoints (DESIGN.md finding 11): the selected candidates that are not markers -- not decoded, or decoded
+// on a level of the candidate hierarchy that identification never reached -- in selection order (descending perimeter), each with
+// the selected quad's own corners (integers, clockwise, neither rotated nor refined).  One block per frame, after k_finish.
+struct RejectedArgs {
+    const int* n_sel;
+    const int* cand_id;
+    FrameScratch fs;
+    int max_raw, max_sel;
+    int32_t* n_rej;  // [F]
+    float* rej;      // [F][max_sel][8]
+};
+
+__global__ void __launch_bounds__(FINISH_THREADS) k_rejected(const RejectedArgs a) {
+    __shared__ short s_parent[FID_MAX_SEL], s_depth[FID_MAX_SEL];
+    __shared__ unsigned char s_was[FID_MAX_SEL];
+    __shared__ short s_src[FID_MAX_SEL];
+    __shared__ int s_n;
+    const int f = blockIdx.x, tid = threadIdx.x;
+    const int ns = a.n_sel[f] < FID_MAX_SEL ? a.n_sel[f] : FID_MAX_SEL;
+    const size_t fo = (size_t)f * a.max_raw;
+    const int* cand_id = a.cand_id + (size_t)f * a.max_sel;
+    for (int i = tid; i < ns; i += FINISH_THREADS) {
+        s_parent[i] = (short)tree_parent(a.fs.quads[fo + a.fs.sel_idx[fo + i]], i, [&](int j) { return a.fs.quads[fo + a.fs.sel_idx[fo + j]]; });
+        s_depth[i] = 0;
+        s_was[i] = 0;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        tree_levels(ns, s_parent, s_depth, s_was, [&](int v) { return cand_id[v] >= 0; });
+        int n = 0;
+        for (int k = 0; k < ns; k++)
+            if (cand_id[k] < 0 || !(s_was[k] & 2)) s_src[n++] = (short)k;
+        s_n = n;
+        a.n_rej[f] = n;
+    }
+    __syncthreads();
+    float* out = a.rej + (size_t)f * a.max_sel * 8;
+    for (int c = tid; c < 4 * s_n; c += FINISH_THREADS) {
+        const QuadF q = a.fs.quads[fo + a.fs.sel_idx[fo + s_src[c >> 2]]];
+        out[2 * c] = q.x[c & 3];
+        out[2 * c + 1] = q.y[c & 3];
+    }
+}
+
+// Poses of the markers k_marker_refine appended in a batch: slots [count[f] - n_rec[f], count[f]) of each frame, solved as k_finish
+// solves the detected ones.  One block per frame, one thread per marker.
+struct RecoveredPoseArgs {
+    const int32_t* count;  // [F] after refinement
+    const int32_t* n_rec;  // [F]
+    const int32_t* ids;
+    const float* corners;
+    int max_markers;
+    Camera cam;
+    double fiducial_len;
+    int n_override;
+    const int32_t* override_ids;
+    const double* override_lens;
+    fid_transform* out_tf;
+};
+
+__global__ void __launch_bounds__(32) k_recovered_pose(const RecoveredPoseArgs a) {
+    const int f = blockIdx.x;
+    const int n = a.count[f];
+    for (int m = n - a.n_rec[f] + (int)threadIdx.x; m < n; m += 32) {
+        const size_t o = (size_t)f * a.max_markers + m;
+        const int id = a.ids[o];
+        double len = (double)(float)a.fiducial_len;
+        for (int k = 0; k < a.n_override; k++)
+            if (a.override_ids[k] == id) len = a.override_lens[k];
+        PoseOut po;
+        solve_marker_pose(a.corners + o * 8, a.cam, (float)len, a.fiducial_len, &po);
+        fid_transform t;
+        t.fiducial_id = id;
+        t.reserved = po.lm_iters;
+        for (int k = 0; k < 3; k++) {
+            t.translation[k] = po.tvec[k];
+            t.rvec[k] = po.rvec[k];
+        }
+        for (int k = 0; k < 4; k++) t.rotation[k] = po.quat[k];
+        t.image_error = po.image_error;
+        t.object_error = po.object_error;
+        t.fiducial_area = po.area;
+        a.out_tf[o] = t;
     }
 }
 

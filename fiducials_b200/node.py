@@ -298,6 +298,43 @@ class Detector:
         left = np.array([r for k, r in enumerate(rej) if k not in taken], np.float32).reshape(-1, 4, 2)
         return oi[: nout.value].copy(), oc[: nout.value].reshape(-1, 4, 2).copy(), left, ri[:nr].copy(), rb[:nr].copy()
 
+    def set_batch_marker_refinement(self, enable: bool):
+        """fid_set_batch_marker_refinement: batches submitted from now on recover missed board markers (with set_marker_refinement
+        enabled and a board set); the recovered markers are appended to each frame's markers."""
+        _lib.check(self.lib.fid_set_batch_marker_refinement(self.h, int(bool(enable))), "fid_set_batch_marker_refinement")
+
+    def last_marker_refinement(self):
+        """fid_last_marker_refinement: for the batch last returned by detect_pose_batch / collect_batch, a list per frame of
+        (recovered_idx, recovered_board, rejected before refinement [m, 4, 2], rejected left [m - n_recovered, 4, 2]) -- the last two
+        as cv2's detectMarkers and refineDetectedMarkers return rejectedImgPoints.  The recovered markers are the frame's last
+        len(recovered_idx) markers."""
+        nf = C.c_int(0)
+        _lib.check(self.lib.fid_last_marker_refinement(self.h, 0, 0, C.byref(nf), None, None, None, None, None), "fid_last_marker_refinement")
+        n = max(nf.value, 1)
+        nrec, nrej = np.zeros(n, np.int32), np.zeros(n, np.int32)
+        _lib.check(self.lib.fid_last_marker_refinement(self.h, 0, 0, C.byref(nf), nrec.ctypes.data_as(C.c_void_p), None, None, nrej.ctypes.data_as(C.c_void_p), None),
+                   "fid_last_marker_refinement")
+        mm, mj = max(int(nrec.max()), 1), max(int(nrej.max()), 1)
+        ri, rb = np.zeros((n, mm), np.int32), np.zeros((n, mm), np.int32)
+        rej = np.zeros((n, mj, 8), np.float32)
+        _lib.check(self.lib.fid_last_marker_refinement(self.h, mm, mj, C.byref(nf), None, ri.ctypes.data_as(C.c_void_p), rb.ctypes.data_as(C.c_void_p), None,
+                                                       rej.ctypes.data_as(C.c_void_p)), "fid_last_marker_refinement")
+        out = []
+        for f in range(nf.value):
+            r, j = int(nrec[f]), int(nrej[f])
+            before = rej[f, :j].reshape(-1, 4, 2).copy()
+            taken = set(ri[f, :r].tolist())
+            left = np.array([q for k, q in enumerate(before) if k not in taken], np.float32).reshape(-1, 4, 2)
+            out.append((ri[f, :r].copy(), rb[f, :r].copy(), before, left))
+        return out
+
+    def debug_rejected(self):
+        """fid_debug_rejected: detectMarkers' rejectedImgPoints [m, 4, 2] for the last detect() call."""
+        n = C.c_int(0)
+        out = np.zeros((_lib.FID_MAX_REJECTED, 8), np.float32)
+        _lib.check(self.lib.fid_debug_rejected(self.h, len(out), C.byref(n), out.ctypes.data_as(C.c_void_p)), "fid_debug_rejected")
+        return out[: n.value].reshape(-1, 4, 2).copy()
+
     def debug_threshold(self, bgr):
         bgr = np.ascontiguousarray(bgr, np.uint8)
         H, W = bgr.shape[:2]
@@ -347,8 +384,10 @@ class FiducialsNode:
 
     def __init__(self, dictionary=7, fiducial_len=0.14, ignore_fiducials: Iterable[int] = (), fiducial_len_override: Optional[Dict[int, float]] = None,
                  do_pose_estimation=True, device=0, max_width=1920, max_height=1080, max_batch=1, doCornerRefinement=True, cornerRefinementSubPix=True, pose_hypotheses=False,
-                 boards=(), charuco_boards=(), **detector_params):
+                 boards=(), charuco_boards=(), refine_markers=None, **detector_params):
         # doCornerRefinement / cornerRefinementSubPix -> cornerRefinementMethod NONE / SUBPIX / CONTOUR (:700-711, configCallback :274-281)
+        if refine_markers is not None and not boards and not charuco_boards:
+            raise ValueError("refine_markers needs boards or charuco_boards")
         detector_params.setdefault("cornerRefinementMethod", (1 if cornerRefinementSubPix else 2) if doCornerRefinement else 0)
         self.fiducial_len = float(fiducial_len)  # :615
         self.doPoseEstimation = do_pose_estimation  # :614
@@ -370,6 +409,15 @@ class FiducialsNode:
         self.charucoBoards = list(charuco_boards)
         if self.charucoBoards:
             self.det.set_charuco_boards(self.charucoBoards)
+        # recovery of missed board markers (new, no reference counterpart): refine_markers = (min_rep_distance, error_correction_rate,
+        # check_all_orders) runs cv2's refineDetectedMarkers against the boards after detection; the recovered markers are reported
+        # like any other marker, and the results carry `recovered` = [(fiducial_id, board)] (board b, or FID_MAX_BOARDS + c for
+        # ChArUco board c)
+        self.refineMarkers = refine_markers is not None
+        if self.refineMarkers:
+            self.det.set_marker_refinement(*refine_markers)
+            self.det.set_batch_marker_refinement(True)
+        self._recovered = []
         self._last_frame = None  # the frame of the last imageCallback, for the ChArUco corners of poseEstimateCallback
         self.haveCamInfo = False
         self.K = None
@@ -401,7 +449,14 @@ class FiducialsNode:
         header = header or Header()
         fva = FiducialArray(header=Header(header.seq, header.stamp, self.frameId))
         try:
-            self.ids, self.corners = self.det.detect(bgr)  # :350
+            if self.refineMarkers:  # the one-frame batch, which refines (detect() is detectMarkers alone)
+                counts, ids, corners, _ = self.det.detect_pose_batch(np.ascontiguousarray(bgr, np.uint8)[None])
+                n = int(counts[0])
+                self.ids, self.corners = ids[0, :n].copy(), corners[0, :n].copy()
+                idx, brd, _, _ = self.det.last_marker_refinement()[0]
+                self._recovered = self._recovered_of(self.ids, idx, brd)
+            else:
+                self.ids, self.corners = self.det.detect(bgr)  # :350
         except _lib.FidError:
             return None  # frame dropped (:389-394)
         if self.charucoBoards:
@@ -411,8 +466,15 @@ class FiducialsNode:
                 continue  # :359-364
             c = self.corners[i]
             fva.fiducials.append(Fiducial(fid, 0, *[float(v) for v in c.reshape(-1)]))  # :366-376
+        if self.refineMarkers:
+            fva.recovered = self._recovered
         self._last_header = header
         return fva
+
+    def _recovered_of(self, ids, idx, boards):
+        """The frame's recovered markers (its last len(idx) markers) as (fiducial_id, board), without the ignored ids."""
+        n0 = len(ids) - len(idx)
+        return [(int(i), int(b)) for i, b in zip(ids[n0:].tolist(), boards.tolist()) if i not in self.ignoreIds]
 
     # :397-538
     def poseEstimateCallback(self, msg: Optional[FiducialArray] = None) -> Optional[FiducialTransformArray]:
@@ -442,6 +504,8 @@ class FiducialsNode:
                 vma.board_poses = boards
             if charuco is not None:
                 vma.charuco = charuco
+            if self.refineMarkers:
+                vma.recovered = self._recovered
             return vma
         for t in tfs:
             if t.fiducial_id in self.ignoreIds:
@@ -453,6 +517,8 @@ class FiducialsNode:
             fta.board_poses = boards
         if charuco is not None:
             fta.charuco = charuco
+        if self.refineMarkers:
+            fta.recovered = self._recovered
         return fta
 
     def _by_id(self, records):
@@ -466,6 +532,7 @@ class FiducialsNode:
         hyps = self.det.last_pose_hypotheses() if self.poseHypotheses else None
         boards = self.det.last_board_poses() if self.boards else None
         charuco = self.det.last_charuco() if self.charucoBoards else None
+        refined = self.det.last_marker_refinement() if self.refineMarkers else None
         out = []
         for f in range(len(counts)):
             fta = FiducialTransformArray(header=Header(0, (0, 0), self.frameId), image_seq=first_seq + f)
@@ -479,6 +546,8 @@ class FiducialsNode:
                 fta.board_poses = boards[f]
             if charuco is not None:
                 fta.charuco = charuco[f]
+            if refined is not None:
+                fta.recovered = self._recovered_of(ids[f, : int(counts[f])], refined[f][0], refined[f][1])
             out.append(fta)
         return out
 

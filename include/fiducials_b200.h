@@ -268,10 +268,27 @@ typedef struct fid_marker_refine_params {
     float error_correction_rate;   /* cv2 default 3; < 0 = no bit check; 0 recovers nothing (the bit test is strict) */
     int32_t check_all_orders;      /* try the 4 corner orders of a candidate (cv2 default 1) */
 } fid_marker_refine_params;
-/* Set the refinement parameters (copied).  The batch calls do not refine in this version; the setting is what
- * fid_refine_detected_markers uses.  FID_ERR_INVALID_ARG for min_rep_distance <= 0 or non-finite values, or while batches are in
- * flight. */
+/* Set the refinement parameters (copied).  fid_refine_detected_markers uses them, and so do the batch calls once
+ * fid_set_batch_marker_refinement is on; this call alone changes nothing in the batch calls.  FID_ERR_INVALID_ARG for
+ * min_rep_distance <= 0 or non-finite values, or while batches are in flight. */
 int fid_set_marker_refinement(fid_detector* h, const fid_marker_refine_params* params);
+/* Refinement inside the batch calls (fid_detect_pose_batch, fid_submit_batch; 0 = off, the default).  A batch refines when this
+ * switch is on, fid_set_marker_refinement is enabled and at least one marker or ChArUco board is set; otherwise it launches exactly
+ * what it launches without the switch.  A refining batch recovers, per frame, the missed board markers from its own rejected list
+ * (fid_debug_rejected's rule) after detection and before the board pose and ChArUco stages, which then see the recovered markers.
+ * Detected markers keep their slots, corners and poses; recovered markers are appended after them in recovery order, with a pose
+ * when the batch has a camera, and counts include them.  When a recovered marker finds no slot below max_markers, the frame stops
+ * refining there and the batch returns FID_ERR_CAPACITY.  fid_detect never refines.  The first enable allocates the buffers.
+ * FID_ERR_INVALID_ARG while batches are in flight. */
+int fid_set_batch_marker_refinement(fid_detector* h, int enable);
+/* The refinement of the batch most recently returned by fid_collect_batch / fid_detect_pose_batch: per frame n_recovered[f],
+ * recovered_idx / recovered_board [f][max_markers] (as fid_refine_detected_markers reports them; the recovered markers are the last
+ * n_recovered[f] of the frame's markers), n_rejected[f] and rejected [f][max_rejected][4][2]: the frame's rejected list BEFORE
+ * refinement, which recovered_idx indexes.  Output pointers may be NULL.  FID_ERR_INVALID_ARG if that batch did not refine;
+ * FID_ERR_CAPACITY, with nothing written, if a frame has more recovered markers than max_markers or more rejected candidates than
+ * max_rejected (for the arrays passed). */
+int fid_last_marker_refinement(fid_detector* h, int max_markers, int max_rejected, int* n_frames, int32_t* n_recovered, int32_t* recovered_idx,
+                               int32_t* recovered_board, int32_t* n_rejected, float* rejected);
 /* refineDetectedMarkers for one frame (in the fid_set_input_encoding format) and lists the caller already has, against every board
  * set: ids / corners hold n detections ([.][4][2] floats) and receive the recovered markers after them (capacity max_markers <=
  * FID_MAX_MARKERS); rejected [n_rejected][4][2] (n_rejected <= FID_MAX_REJECTED) is detectMarkers' rejectedImgPoints.  cam may be
@@ -326,6 +343,11 @@ int fid_debug_time_threshold(fid_detector* h, int n_frames, const uint8_t* bgr_d
  * (scale-major, contour-list order): quads[n*8] int32 vertices (approxPolyDP order), scale[n],
  * contour_len[n]. */
 int fid_debug_candidates(fid_detector* h, int max_candidates, int* n, int32_t* quads, int32_t* scale, int32_t* contour_len);
+/* detectMarkers' rejectedImgPoints for the last fid_detect call on slot 0: the selected candidates that are not markers (not
+ * decoded, or never reached by OpenCV 4.13's candidate hierarchy), in selection order (descending perimeter), each with its own
+ * integer corners in the clockwise order of the candidate stage, neither rotated nor refined.  rejected [n][4][2] floats (may be
+ * NULL).  *n = the count; FID_ERR_CAPACITY if it exceeds max_rejected; FID_ERR_INVALID_ARG before the handle's first fid_detect. */
+int fid_debug_rejected(fid_detector* h, int max_rejected, int* n, float* rejected);
 
 /* Per-stage device times (milliseconds, CUDA events) of the last batch call:
  * [0] h2d copy, [1] threshold (+ start cracks), [2] unused (reads 0), [3] border walk, [4] chain emit, [5] polygon+filters,

@@ -3,8 +3,8 @@
 128 rendered 1080p frames, each with a 10 x 7 GridBoard of DICT_6X6_250 (40 mm markers, 10 mm gaps) warped in at a seeded pose and
 three of its markers' inner bits painted over; cv2's detectMarkers gives each frame's detected and rejected lists.  Under
 torch.profiler, one fid_refine_detected_markers call per frame (with a camera), after a warm-up pass: the device time of
-k_marker_refine summed over the 128 frames, and the markers recovered.  The batch calls do not refine, so there is no frames/s
-comparison to make yet.
+k_marker_refine summed over the 128 frames, and the markers recovered.  The batch path and its frames/s are measured by
+tools/bench_batch_refine.py.
 
 Prints the card name and power limit read in the same run; --out DIR also writes the numbers as JSON.
     python tools/bench_marker_refine.py [--frames 128] [--out DIR]"""
