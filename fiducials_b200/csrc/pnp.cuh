@@ -411,14 +411,18 @@ FID_HD void solve_marker_pose(const float corners[8], const Camera& cam, float m
     // 1. normalise + undistort
     double mn[4][2];
     for (int i = 0; i < 4; i++) undistort_point(img[2 * i], img[2 * i + 1], cam, mn[i]);
-    // 2-4. planar initialisation (object plane is z=0 with zero centroid => Rt = I, Tt = 0)
-    double src[4][2];
+    // 2-4. planar initialisation (object plane is z=0 with zero centroid => Rt = I, Tt = 0).  findHomography converts
+    // both point sets to float32 (board_pnp.cuh does the same); the object points already are.  Without the rounding the
+    // homography moves by ~1e-6, enough to pick the other branch of rodrigues_m2v near a half turn (DESIGN findings 7, 12).
+    double src[4][2], dst[4][2];
     for (int i = 0; i < 4; i++) {
         src[i][0] = obj[i][0];
         src[i][1] = obj[i][1];
+        dst[i][0] = (float)mn[i][0];
+        dst[i][1] = (float)mn[i][1];
     }
     double Hm[9];
-    homography4(src, mn, Hm);
+    homography4(src, dst, Hm);
     double h1[3] = {Hm[0], Hm[3], Hm[6]}, h2[3] = {Hm[1], Hm[4], Hm[7]}, h3[3] = {Hm[2], Hm[5], Hm[8]};
     const double n1 = sqrt(h1[0] * h1[0] + h1[1] * h1[1] + h1[2] * h1[2]);
     const double n2 = sqrt(h2[0] * h2[0] + h2[1] * h2[1] + h2[2] * h2[2]);
