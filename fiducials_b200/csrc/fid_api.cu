@@ -68,6 +68,8 @@ struct Slot {
     int32_t* d_mr_nrec = nullptr;                      // [max_batch]                 k_marker_refine
     int32_t* d_mr_idx = nullptr;                       // [max_batch][max_markers]
     int32_t* d_mr_board = nullptr;                     // [max_batch][max_markers]
+    int32_t* d_dia_n = nullptr;                        // fid_set_diamonds: [max_batch], allocated by the first enable
+    fid_diamond* d_dia = nullptr;                      // [max_batch][FID_MAX_DIAMONDS]
     // pinned host mirrors
     int32_t* h_out_count = nullptr;
     int32_t* h_out_ids = nullptr;
@@ -84,6 +86,8 @@ struct Slot {
     int32_t* h_mr_nrec = nullptr;
     int32_t* h_mr_idx = nullptr;
     int32_t* h_mr_board = nullptr;
+    int32_t* h_dia_n = nullptr;
+    fid_diamond* h_dia = nullptr;
     Counters* h_counters = nullptr;
     int* h_nsel = nullptr;
     int* h_nrawc = nullptr;
@@ -113,7 +117,7 @@ struct fid_detector {
     struct Pending {
         int first_slot, n_chunks, n_frames, w, h;
         int64_t launches;
-        bool pose, hyp, board, charuco, refine;
+        bool pose, hyp, board, charuco, refine, diamonds;
     } pending[MAX_SLOTS]{};
     int pend_head = 0, pend_count = 0, slots_in_use = 0, slot_next = 0;
     cudaStream_t slot_stream[MAX_SLOTS] = {};
@@ -181,6 +185,15 @@ struct fid_detector {
     std::vector<int32_t> last_mr_nrec, last_mr_nrej;  // [last_mr_frames]
     std::vector<int32_t> last_mr_idx, last_mr_board;  // frame after frame, last_mr_nrec[f] each
     std::vector<float> last_mr_rej;                   // frame after frame, last_mr_nrej[f] x 8 each
+    // ChArUco diamonds (fid_set_diamonds / fid_detect_diamonds / fid_last_diamonds)
+    fid_diamond_params diamond{};                    // enable = 0: off
+    DiamondLayout diamond_layout{};
+    int32_t* d_dia_io = nullptr;                     // fid_detect_diamonds: the list's length, the diamonds found
+    fid_diamond* d_dia_list = nullptr;               // fid_detect_diamonds output, FID_MAX_DIAMONDS records
+    bool last_dia_valid = false;                     // the batch last returned had diamonds (fid_last_diamonds)
+    int last_dia_frames = 0;
+    std::vector<int32_t> last_dia_n;                 // [last_dia_frames]
+    std::vector<fid_diamond> last_dia;               // frame after frame, last_dia_n[f] each
     int32_t* d_dbg_rej_n = nullptr;                  // fid_debug_rejected: count, then [max_sel][8] floats
     float* d_dbg_rej = nullptr;
     float stage_ms[ST_COUNT + N_WALK_ROUNDS]{};
@@ -369,11 +382,11 @@ static void free_slot(Slot& s) {
                      s.fs.group_members, s.fs.next_in_group, s.fs.group_head, s.fs.group_tail, s.fs.close_count, s.fs.close_idx,   s.fs.close_off,  s.fs.selected,
                      s.fs.sel_idx,    s.d_nsel,          s.d_nrawc,         s.d_cand_id,      s.d_cand_corners, s.d_out_count,    s.d_out_ids,     s.d_out_corners,
                      s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp, s.d_out_board, s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy,
-                     s.d_rej_n,       s.d_rej,           s.d_mr_nrec,       s.d_mr_idx,       s.d_mr_board};
+                     s.d_rej_n,       s.d_rej,           s.d_mr_nrec,       s.d_mr_idx,       s.d_mr_board,    s.d_dia_n,       s.d_dia};
     for (void* p : dptrs)
         if (p) cudaFree(p);
     void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp, s.h_out_board, s.h_out_ch, s.h_out_ch_ids, s.h_out_ch_xy,
-                     s.h_rej_n,     s.h_rej,     s.h_mr_nrec,    s.h_mr_idx,   s.h_mr_board};
+                     s.h_rej_n,     s.h_rej,     s.h_mr_nrec,    s.h_mr_idx,   s.h_mr_board, s.h_dia_n, s.h_dia};
     for (void* p : hptrs)
         if (p) cudaFreeHost(p);
     for (int i = 0; i <= ST_COUNT; i++)
@@ -526,7 +539,7 @@ extern "C" int fid_destroy(fid_detector* h) {
     void* ptrs[] = {h->d_prune, h->d_dict, h->d_pf[0], h->d_pf[1], h->d_lut_prev, h->d_lut_next, h->d_subpix_masks, h->d_override_ids, h->d_override_lens, h->d_pose_ids, h->d_pose_corners, h->d_pose_out, h->d_hyp_list,
                      h->d_board_off, h->d_board_keys, h->d_board_marker, h->d_board_obj, h->d_board_count, h->d_board_list, h->d_ch_boards, h->d_ch_keys,
                      h->d_ch_marker, h->d_ch_ids, h->d_ch_near_n, h->d_ch_near_idx, h->d_ch_near_corner, h->d_ch_obj, h->d_ch_chess, h->d_ch_masks,
-                     h->d_ch_count, h->d_ch_list, h->d_ch_list_ids, h->d_ch_list_xy, h->d_mr_i, h->d_mr_f, h->d_dbg_rej_n, h->d_dbg_rej};
+                     h->d_ch_count, h->d_ch_list, h->d_ch_list_ids, h->d_ch_list_xy, h->d_mr_i, h->d_mr_f, h->d_dbg_rej_n, h->d_dbg_rej, h->d_dia_io, h->d_dia_list};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     for (int i = 0; i < 2; i++)
@@ -683,11 +696,33 @@ static MarkerRefineArgs marker_refine_args(const fid_detector* h, const uint8_t*
     return a;
 }
 
+// k_diamond's frames and parameters; the caller sets the lists.
+static DiamondArgs diamond_args(const fid_detector* h, const uint8_t* src, size_t row_stride, size_t frame_stride, int W, int H, const fid_camera* cam) {
+    DiamondArgs a{};
+    a.src = src;
+    a.row_stride = row_stride;
+    a.frame_stride = frame_stride;
+    a.enc = h->enc;
+    a.W = W;
+    a.H = H;
+    a.P = h->P;
+    a.subpix_masks = h->d_subpix_masks;
+    a.ch_masks = h->d_ch_masks;
+    a.layout = h->diamond_layout;
+    a.win_default = std::max(1, std::min(FID_CHARUCO_MAX_WIN, h->params.cornerRefinementWinSize));  // as charuco_args
+    a.max_iters = std::max(1, std::min(100, h->params.cornerRefinementMaxIterations));
+    const double eps = std::max(h->params.cornerRefinementMinAccuracy, 0.0);
+    a.eps_sq = eps * eps;
+    a.has_cam = cam ? 1 : 0;
+    a.cam = make_camera(cam);
+    return a;
+}
+
 // A batch refines only with the batch switch, the refinement parameters and a board to refine against.
 static bool batch_refines(const fid_detector* h) { return h->batch_refine && h->mrefine.enable && h->n_boards + h->n_charuco > 0; }
 
 static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, const FrameGeom& g, const uint8_t* d_bgr, const fid_camera* cam, double fiducial_len,
-                            int n_override, int stop_after /* -1 = all */, const Slot* prev = nullptr, bool refine = false) {
+                            int n_override, int stop_after /* -1 = all */, const Slot* prev = nullptr, bool refine = false, bool diamonds = false) {
     const DevParams& P = h->P;
     const int W = g.W, H = g.H;
     int launches = 0;
@@ -1030,14 +1065,27 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
                                  s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy));
         launches++;
     }
+    if (diamonds) {  // opt-in: ChArUco diamonds per frame, from the final markers (fid_set_diamonds)
+        DiamondArgs a = diamond_args(h, d_bgr, g.bgr_row_stride, g.bgr_frame_stride, W, H, cam);
+        a.max_markers = h->max_markers;
+        a.count = s.d_out_count;
+        a.ids = s.d_out_ids;
+        a.corners = s.d_out_corners;
+        a.n_out = s.d_dia_n;
+        a.out = s.d_dia;
+        launch_prio(k_diamond, dim3(nf), dim3(DIAMOND_THREADS), 0, st, 5, a);
+        launches++;
+    }
     CK(cudaEventRecord(s.ev[ST_D2H], st));
     h->counters[6] += launches;
     CK(cudaGetLastError());
     return FID_OK;
 }
 
-static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose, bool with_hyp, bool with_board, bool with_charuco, bool with_refine) {
+static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose, bool with_hyp, bool with_board, bool with_charuco, bool with_refine,
+                       bool with_diamonds) {
     const size_t M = (size_t)nf * h->max_markers;
+    if (with_diamonds) CK(cudaMemcpyAsync(s.h_dia_n, s.d_dia_n, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));  // collect copies the records
     if (with_refine) {  // counts only: collect copies the lists at their lengths
         CK(cudaMemcpyAsync(s.h_rej_n, s.d_rej_n, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(s.h_mr_nrec, s.d_mr_nrec, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));
@@ -1062,9 +1110,22 @@ static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool w
 }
 
 static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* tfs, bool first_chunk,
-                   struct fid_pose_hypotheses* hyps = nullptr, fid_board_pose* boards = nullptr, int ch_first = -1, bool refined = false) {
+                   struct fid_pose_hypotheses* hyps = nullptr, fid_board_pose* boards = nullptr, int ch_first = -1, bool refined = false, bool diamonds = false) {
     CK(cudaEventSynchronize(s.done));
     int status = FID_OK;
+    if (diamonds) {  // the diamond records (fid_last_diamonds), each row at the frame with the most diamonds
+        int max_d = 0;
+        for (int f = 0; f < nf; f++) max_d = std::max(max_d, (int)s.h_dia_n[f]);
+        if (max_d) {
+            const cudaStream_t st = h->slot_stream[&s - h->slot];
+            CK(cudaMemcpy2DAsync(s.h_dia, sizeof(fid_diamond) * max_d, s.d_dia, sizeof(fid_diamond) * FID_MAX_DIAMONDS, sizeof(fid_diamond) * max_d, nf, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+        }
+        for (int f = 0; f < nf; f++) {
+            h->last_dia_n.push_back(s.h_dia_n[f]);
+            h->last_dia.insert(h->last_dia.end(), s.h_dia + (size_t)f * max_d, s.h_dia + (size_t)f * max_d + s.h_dia_n[f]);
+        }
+    }
     if (refined) {  // the rejected lists and the recovered markers (fid_last_marker_refinement), each row at the longest frame's length
         const cudaStream_t st = h->slot_stream[&s - h->slot];
         int max_rej = 0, max_rec = 0;
@@ -1199,7 +1260,16 @@ static void begin_last_refinement(fid_detector* h, bool refine, int n_frames) {
     h->last_mr_rej.clear();
 }
 
-// fid_detect_pose_batch; fid_detect (detectMarkers) passes may_refine = false.
+// The same for the diamonds (fid_last_diamonds); collect appends frame after frame.
+static void begin_last_diamonds(fid_detector* h, bool dia, int n_frames) {
+    h->last_dia_valid = false;
+    if (!dia) return;
+    h->last_dia_frames = n_frames;
+    h->last_dia_n.clear();
+    h->last_dia.clear();
+}
+
+// fid_detect_pose_batch; fid_detect (detectMarkers) passes may_refine = false, which also leaves diamonds out.
 static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
                              const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
                              int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms, bool may_refine) {
@@ -1223,6 +1293,8 @@ static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, 
     begin_last_charuco(h, chr, n_frames);
     const bool mr = may_refine && batch_refines(h);
     begin_last_refinement(h, mr, n_frames);
+    const bool dia = may_refine && h->diamond.enable;
+    begin_last_diamonds(h, dia, n_frames);
     h->counters[6] = 0;
     h->stage_ms[ST_H2D] = 0;
     // software pipeline over chunks: up to n_slots chunks in flight, each on its own stream; results of
@@ -1273,9 +1345,9 @@ static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, 
                 h->pf_h = height;
                 h->hint_next = nullptr;
             }
-            rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, c > 0 ? &h->slot[(c - 1) % NS] : nullptr, mr);
+            rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, c > 0 ? &h->slot[(c - 1) % NS] : nullptr, mr, dia);
             if (rc != FID_OK) return rc;
-            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp, brd, chr, mr);
+            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp, brd, chr, mr, dia);
             if (rc != FID_OK) return rc;
             h->last_frames = nf;
         }
@@ -1285,7 +1357,7 @@ static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, 
             const int nf = std::min(B, n_frames - pc * B);
             rc = collect(h, s, nf, max_markers, counts + (size_t)pc * B, ids ? ids + (size_t)pc * B * max_markers : nullptr,
                          corners ? corners + (size_t)pc * B * max_markers * 8 : nullptr, (transforms && cam) ? transforms + (size_t)pc * B * max_markers : nullptr, pc == 0,
-                         hyps ? hyps + (size_t)pc * B * max_markers : nullptr, boards ? boards + (size_t)pc * B * h->n_boards : nullptr, chr ? pc * B : -1, mr);
+                         hyps ? hyps + (size_t)pc * B * max_markers : nullptr, boards ? boards + (size_t)pc * B * h->n_boards : nullptr, chr ? pc * B : -1, mr, dia);
             if (rc != FID_OK) status = rc;
         }
     }
@@ -1293,6 +1365,7 @@ static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, 
     h->last_board_valid = brd;
     h->last_ch_valid = chr;
     h->last_mr_valid = mr;
+    h->last_dia_valid = dia;
     return status;
 }
 
@@ -1321,6 +1394,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
     const bool contiguous = row_stride == (size_t)width * h->bpp && frame_stride == row_stride * height;
     const int first = h->slot_next;
     const bool mr = batch_refines(h);
+    const bool dia = h->diamond.enable != 0;
     h->counters[6] = 0;
     for (int c = 0; c < n_chunks; c++) {
         const int si = (first + c) % NS;
@@ -1347,9 +1421,9 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
             g = make_geom(h, width, height, (size_t)width * h->bpp, (size_t)width * h->bpp * height);
         }
         const Slot* prev = (h->slots_in_use + c) > 0 ? &h->slot[(si + NS - 1) % NS] : nullptr;
-        rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, prev, mr);
+        rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, prev, mr, dia);
         if (rc != FID_OK) return rc;
-        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam, h->n_boards && cam, h->n_charuco > 0, mr);
+        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam, h->n_boards && cam, h->n_charuco > 0, mr, dia);
         if (rc != FID_OK) return rc;
         h->last_frames = nf;
     }
@@ -1364,6 +1438,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
     pb.board = h->n_boards && cam;
     pb.charuco = h->n_charuco > 0;
     pb.refine = mr;
+    pb.diamonds = dia;
     pb.launches = h->counters[6];
     h->pend_count++;
     h->slots_in_use += n_chunks;
@@ -1383,19 +1458,21 @@ extern "C" int fid_collect_batch(fid_detector* h, int max_markers, int32_t* coun
     fid_board_pose* boards = begin_last_boards(h, pb.board, pb.n_frames);
     begin_last_charuco(h, pb.charuco, pb.n_frames);
     begin_last_refinement(h, pb.refine, pb.n_frames);
+    begin_last_diamonds(h, pb.diamonds, pb.n_frames);
     for (int c = 0; c < pb.n_chunks; c++) {
         Slot& s = h->slot[(pb.first_slot + c) % NS];
         const int nf = std::min(B, pb.n_frames - c * B);
         const int rc = collect(h, s, nf, max_markers, counts + (size_t)c * B, ids ? ids + (size_t)c * B * max_markers : nullptr,
                                corners ? corners + (size_t)c * B * max_markers * 8 : nullptr, (transforms && pb.pose) ? transforms + (size_t)c * B * max_markers : nullptr, c == 0,
                                hyps ? hyps + (size_t)c * B * max_markers : nullptr, boards ? boards + (size_t)c * B * h->n_boards : nullptr,
-                               pb.charuco ? c * B : -1, pb.refine);
+                               pb.charuco ? c * B : -1, pb.refine, pb.diamonds);
         if (rc != FID_OK) status = rc;
     }
     end_last_hypotheses(h, pb.hyp, counts);
     h->last_board_valid = pb.board;
     h->last_ch_valid = pb.charuco;
     h->last_mr_valid = pb.refine;
+    h->last_dia_valid = pb.diamonds;
     h->pend_head = (h->pend_head + 1) % MAX_SLOTS;
     h->pend_count--;
     h->slots_in_use -= pb.n_chunks;
@@ -1829,6 +1906,86 @@ extern "C" int fid_last_marker_refinement(fid_detector* h, int max_markers, int 
         if (rejected) memcpy(rejected + (size_t)f * max_rejected * 8, h->last_mr_rej.data() + oj * 8, sizeof(float) * 8 * nj);
         oi += nr;
         oj += nj;
+    }
+    return FID_OK;
+}
+
+extern "C" int fid_set_diamonds(fid_detector* h, const fid_diamond_params* params) {
+    if (!h || !params || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight read the layout
+    const fid_diamond_params p = *params;
+    DiamondLayout L{};
+    if (p.enable) {
+        if (!std::isfinite(p.square_length) || !(p.marker_length > 0) || !(p.marker_length < p.square_length)) return FID_ERR_INVALID_ARG;
+        if (p.min_markers < 0 || p.min_markers > 2) return FID_ERR_INVALID_ARG;  // cv2 asserts outside 0..2
+        if (!diamond_layout(p.square_length, p.marker_length, p.min_markers, p.check_markers ? 1 : 0, &L)) return FID_ERR_INVALID_ARG;
+        CK(cudaSetDevice(h->device));
+        int rc;  // (a failed allocation leaves the option off; the next enable completes it)
+        for (int i = 0; i < h->n_slots; i++) {
+            Slot& s = h->slot[i];
+            if (!s.d_dia_n && (rc = dalloc(&s.d_dia_n, (size_t)h->max_batch)) != FID_OK) return rc;
+            if (!s.d_dia && (rc = dalloc(&s.d_dia, (size_t)h->max_batch * FID_MAX_DIAMONDS)) != FID_OK) return rc;
+            if (!s.h_dia_n && (rc = halloc(&s.h_dia_n, (size_t)h->max_batch)) != FID_OK) return rc;
+            if (!s.h_dia && (rc = halloc(&s.h_dia, (size_t)h->max_batch * FID_MAX_DIAMONDS)) != FID_OK) return rc;
+        }
+        if (!h->d_dia_io && (rc = dalloc(&h->d_dia_io, 2)) != FID_OK) return rc;
+        if (!h->d_dia_list && (rc = dalloc(&h->d_dia_list, FID_MAX_DIAMONDS)) != FID_OK) return rc;
+        if (!h->d_ch_masks) {  // the chessboard corners' cornerSubPix table, shared with the ChArUco boards
+            std::vector<float> masks(FID_CHARUCO_MASK_FLOATS);
+            charuco_subpix_masks(masks.data());
+            if ((rc = dalloc(&h->d_ch_masks, masks.size())) != FID_OK) return rc;
+            CK(cudaMemcpy(h->d_ch_masks, masks.data(), sizeof(float) * masks.size(), cudaMemcpyHostToDevice));
+            CK(cudaFuncSetAttribute(k_charuco, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CHARUCO_SMEM));
+        }
+    }
+    h->diamond = p;
+    h->diamond.enable = p.enable ? 1 : 0;
+    h->diamond_layout = L;
+    return FID_OK;
+}
+
+extern "C" int fid_detect_diamonds(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int n, const int32_t* ids, const float* corners,
+                                   const fid_camera* cam, int* n_diamonds, fid_diamond* out) {
+    if (!h || !bgr || !n_diamonds || n < 0 || n > FID_MAX_MARKERS || (n > 0 && (!ids || !corners)) || (n >= 4 && !out) || !h->diamond.enable) return FID_ERR_INVALID_ARG;
+    if (width < 16 || height < 16 || width > h->max_w || height > h->max_h || stride < (size_t)width * h->bpp) return FID_ERR_INVALID_ARG;
+    if (h->pend_count) return FID_ERR_INVALID_ARG;  // slot 0 may belong to a batch in flight
+    CK(cudaSetDevice(h->device));
+    Slot& s = h->slot[0];
+    CK(cudaMemcpy2DAsync(s.d_bgr, (size_t)width * h->bpp, bgr, stride, (size_t)width * h->bpp, height, cudaMemcpyHostToDevice, h->stream));
+    if (n > 0) {
+        CK(cudaMemcpyAsync(h->d_pose_ids, ids, sizeof(int32_t) * n, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(h->d_pose_corners, corners, sizeof(float) * 8 * n, cudaMemcpyHostToDevice, h->stream));
+    }
+    CK(cudaMemcpyAsync(h->d_dia_io, &n, sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+    DiamondArgs a = diamond_args(h, s.d_bgr, (size_t)width * h->bpp, (size_t)width * h->bpp * height, width, height, cam);
+    a.max_markers = FID_MAX_MARKERS;
+    a.count = h->d_dia_io;
+    a.ids = h->d_pose_ids;
+    a.corners = h->d_pose_corners;
+    a.n_out = h->d_dia_io + 1;
+    a.out = h->d_dia_list;
+    k_diamond<<<1, DIAMOND_THREADS, 0, h->stream>>>(a);
+    CK(cudaGetLastError());
+    int32_t nd = 0;
+    CK(cudaMemcpyAsync(&nd, h->d_dia_io + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (nd > 0) CK(cudaMemcpy(out, h->d_dia_list, sizeof(fid_diamond) * nd, cudaMemcpyDeviceToHost));
+    *n_diamonds = nd;
+    return FID_OK;
+}
+
+extern "C" int fid_last_diamonds(fid_detector* h, int max_diamonds, int* n_frames, int32_t* counts, fid_diamond* out) {
+    if (!h || max_diamonds < 0 || !h->last_dia_valid) return FID_ERR_INVALID_ARG;
+    const int nf = h->last_dia_frames;
+    if (out)
+        for (int f = 0; f < nf; f++)
+            if (h->last_dia_n[f] > max_diamonds) return FID_ERR_CAPACITY;
+    if (n_frames) *n_frames = nf;
+    size_t o = 0;
+    for (int f = 0; f < nf; f++) {
+        const int nd = h->last_dia_n[f];
+        if (counts) counts[f] = nd;
+        if (out) memcpy(out + (size_t)f * max_diamonds, h->last_dia.data() + o, sizeof(fid_diamond) * nd);
+        o += nd;
     }
     return FID_OK;
 }

@@ -12,6 +12,7 @@
 //   k_marker_refine  one block per frame: board markers recovered from the rejected candidates (marker_refine.cuh)
 //   k_rejected    opt-in, after k_finish: one block per frame, detectMarkers' rejected list (candidate_tree.cuh)
 //   k_recovered_pose  opt-in, after k_marker_refine in a batch: the poses of the recovered markers
+//   k_diamond     opt-in, last: one block per frame, its ChArUco diamonds and their poses (diamond.cuh)
 #pragma once
 #include <cuda_runtime.h>
 
@@ -21,6 +22,7 @@
 #include "charuco.cuh"
 #include "common.cuh"
 #include "contour_refine.cuh"
+#include "diamond.cuh"
 #include "identify.cuh"
 #include "ippe.cuh"
 #include "marker_refine.cuh"
@@ -1416,6 +1418,138 @@ __global__ void __launch_bounds__(MREFINE_THREADS) k_marker_refine(const MarkerR
     if (tid == 0) {
         a.count[f] = s_n;
         a.n_rec[f] = s_nrec;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// ChArUco diamonds (diamond.cuh), an opt-in stage of its own after every other stage.  It reads the frame's final marker list and
+// leaves it unchanged: the loop's cornerSubPix write-backs go to a copy in shared memory.
+struct DiamondArgs {
+    const uint8_t* src;
+    size_t row_stride, frame_stride;
+    int enc, W, H;
+    DevParams P;
+    const float* subpix_masks;  // windows 1..5 (k_finish's table)
+    const float* ch_masks;      // charuco_subpix_masks
+    DiamondLayout layout;
+    int win_default, max_iters;  // as CharucoArgs
+    double eps_sq;
+    int has_cam;
+    Camera cam;
+    int max_markers;
+    const int32_t* count;   // [F]                     the markers (k_finish, k_marker_refine, or one host list)
+    const int32_t* ids;     // [F][max_markers]
+    const float* corners;   // [F][max_markers][8]
+    int32_t* n_out;         // [F]
+    fid_diamond* out;       // [F][FID_MAX_DIAMONDS]
+};
+
+#define DIAMOND_THREADS 128
+#define DIAMOND_WARPS (DIAMOND_THREADS / 32)
+
+// One block per frame.  The warps predict every marker's three neighbours (they depend on that marker alone), warp 0 replays the
+// order-dependent loop with lane-parallel candidate screens, predicting again only markers whose corners a recovery refined, then a
+// warp per diamond finds its chessboard corners (approximate pose with a camera, a lane per corner, the board check), and a thread
+// per kept diamond, in loop order, solves its pose.
+__global__ void __launch_bounds__(DIAMOND_THREADS) k_diamond(const DiamondArgs a) {
+    __shared__ float s_wc[FID_MAX_MARKERS * 8];
+    __shared__ float s_pred[FID_MAX_MARKERS * 24];
+    __shared__ uint8_t s_ok[FID_MAX_MARKERS], s_dirty[FID_MAX_MARKERS], s_taken[FID_MAX_MARKERS];
+    __shared__ int32_t s_dia[FID_MAX_DIAMONDS * 4], s_pos[FID_MAX_DIAMONDS];
+    __shared__ float s_xy[FID_MAX_DIAMONDS * 8];
+    __shared__ float s_det[DIAMOND_WARPS][32];
+    __shared__ double s_mn[DIAMOND_WARPS][32];
+    __shared__ DiamondLayout s_L;
+    __shared__ int s_nd;
+    const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int n = min(a.count[f], min(a.max_markers, FID_MAX_MARKERS));
+    const int32_t* ids = a.ids + (size_t)f * a.max_markers;
+    const float* corners = a.corners + (size_t)f * a.max_markers * 8;
+    const FrameImg gray{a.src + (size_t)f * a.frame_stride, a.row_stride, a.enc};
+    for (int c = tid; c < 8 * n; c += DIAMOND_THREADS) s_wc[c] = corners[c];
+    if (tid == 0) s_L = a.layout;
+    __syncthreads();
+    // 1. a warp per marker: its predictions from the corners as detected
+    for (int i = warp; n >= 4 && i < n; i += DIAMOND_WARPS) {
+        float pr[24];
+        const bool ok = diamond_predict(s_L, s_wc + 8 * i, pr);
+        if (lane == 0) {
+            s_ok[i] = ok;
+            for (int k = 0; k < 24; k++) s_pred[24 * i + k] = pr[k];
+        }
+    }
+    __syncthreads();
+    // 2. warp 0: the loop
+    if (warp == 0) {
+        const int nd = diamond_assign(WarpLanes{}, gray, a.W, a.H, a.P, a.subpix_masks, s_L, n, s_wc, s_pred, s_ok, s_dirty, s_taken, s_dia);
+        if (lane == 0) s_nd = nd;
+    }
+    __syncthreads();
+    const int nd = s_nd;
+    // 3. a warp per diamond: its chessboard corners
+    for (int k = warp; k < nd; k += DIAMOND_WARPS) {
+        const int32_t* m = s_dia + 4 * k;
+        float* det = s_det[warp];
+        det[lane] = s_wc[8 * m[lane >> 3] + (lane & 7)];
+        __syncwarp();
+        int32_t tmp[4];
+        diamond_tmp_ids(ids[m[0]], tmp);
+        const CharucoView B = diamond_view(s_L, tmp);
+        double R[9], p[6];
+        if (a.has_cam) {
+            BoardPoseOut po;
+            solve_board_pose(16, s_L.obj, det, s_mn[warp], a.cam, &po);
+            for (int j = 0; j < 3; j++) {
+                p[j] = po.rvec[j];
+                p[3 + j] = po.tvec[j];
+            }
+            rodrigues_v2m(p, R, nullptr);
+        }
+        float xy[2] = {-1.f, -1.f};
+        bool keep = true;
+        if (lane < 4) {
+            float patch[(2 * FID_CHARUCO_MAX_WIN + 3) * (2 * FID_CHARUCO_MAX_WIN + 3)];
+            keep = diamond_corner(B, lane, a.has_cam != 0, R, p, a.cam, gray, a.W, a.H, det, a.ch_masks, a.win_default, a.max_iters, a.eps_sq, patch, xy);
+        }
+        bool all = __all_sync(0xffffffffu, keep);
+        if (all && s_L.check_markers && lane < 4) keep = charuco_check_corner(B, lane, xy, 4, tmp, s_L.rows, det);
+        all = __all_sync(0xffffffffu, keep);
+        if (lane < 4) {
+            s_xy[8 * k + 2 * diamond_slot(lane)] = xy[0];
+            s_xy[8 * k + 2 * diamond_slot(lane) + 1] = xy[1];
+        }
+        if (lane == 0) s_pos[k] = all;
+        __syncwarp();
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int q = 0;
+        for (int k = 0; k < nd; k++) s_pos[k] = s_pos[k] ? q++ : -1;
+        a.n_out[f] = q;
+    }
+    __syncthreads();
+    // 4. a thread per kept diamond: the record and the pose
+    for (int k = tid; k < nd; k += DIAMOND_THREADS) {
+        if (s_pos[k] < 0) continue;
+        fid_diamond r{};
+        for (int j = 0; j < 4; j++) r.ids[j] = ids[s_dia[4 * k + j]];
+        for (int j = 0; j < 8; j++) r.corners[j] = s_xy[8 * k + j];
+        r.pose.fiducial_id = r.ids[0];
+        if (a.has_cam) {
+            PoseOut po;
+            solve_marker_pose(r.corners, a.cam, s_L.square_length, (double)s_L.square_length, &po);
+            r.status = 1;
+            r.pose.reserved = po.lm_iters;
+            for (int j = 0; j < 3; j++) {
+                r.pose.translation[j] = po.tvec[j];
+                r.pose.rvec[j] = po.rvec[j];
+            }
+            for (int j = 0; j < 4; j++) r.pose.rotation[j] = po.quat[j];
+            r.pose.image_error = po.image_error;
+            r.pose.object_error = po.object_error;
+            r.pose.fiducial_area = po.area;
+        }
+        a.out[(size_t)f * FID_MAX_DIAMONDS + s_pos[k]] = r;
     }
 }
 

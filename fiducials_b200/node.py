@@ -328,6 +328,48 @@ class Detector:
             out.append((ri[f, :r].copy(), rb[f, :r].copy(), before, left))
         return out
 
+    def set_diamonds(self, square_length, marker_length=None, min_markers=2, check_markers=True):
+        """fid_set_diamonds: the ChArUco diamond geometry (square_length=None turns diamonds off).  Batches submitted from now on also
+        find each frame's diamonds (and, with a camera, their poses)."""
+        p = _lib.fid_diamond_params()
+        if square_length is not None:
+            p.enable, p.square_length, p.marker_length = 1, square_length, marker_length
+            p.min_markers, p.check_markers = int(min_markers), int(bool(check_markers))
+        _lib.check(self.lib.fid_set_diamonds(self.h, C.byref(p)), "fid_set_diamonds")
+
+    @staticmethod
+    def _diamond_split(recs):
+        """(ids [k, 4] int32, corners [k, 4, 2] float32, fid_diamond records) -- cv2's diamondIds and diamondCorners, and the poses."""
+        ids = np.array([list(r.ids) for r in recs], np.int32).reshape(-1, 4)
+        corners = np.array([list(r.corners) for r in recs], np.float32).reshape(-1, 4, 2)
+        return ids, corners, list(recs)
+
+    def diamonds(self, frame, ids, corners, K=None, D=None):
+        """fid_detect_diamonds: the diamonds of one frame among markers already detected (ids, corners as detect()), as
+        cv2.aruco.CharucoDetector.detectDiamonds finds them.  Without K no pose.  Returns (ids, corners, records)."""
+        frame = np.ascontiguousarray(frame, np.uint8)
+        H, W = frame.shape[:2]
+        ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+        corners = np.ascontiguousarray(corners, np.float32).reshape(-1, 8)
+        out = (_lib.fid_diamond * max(len(ids) // 4, 1))()
+        nd = C.c_int(0)
+        cam = None if K is None else C.byref(_camera(K, D))
+        _lib.check(self.lib.fid_detect_diamonds(self.h, frame.ctypes.data_as(C.c_void_p), W, H, frame.strides[0], len(ids), ids.ctypes.data_as(C.c_void_p),
+                                                corners.ctypes.data_as(C.c_void_p), cam, C.byref(nd), C.cast(out, C.c_void_p)), "fid_detect_diamonds")
+        return self._diamond_split([out[i] for i in range(nd.value)])
+
+    def last_diamonds(self):
+        """fid_last_diamonds: for the batch last returned by detect_pose_batch / collect_batch, a list per frame of (ids, corners,
+        records) as diamonds() returns them."""
+        nf = C.c_int(0)
+        _lib.check(self.lib.fid_last_diamonds(self.h, 0, C.byref(nf), None, None), "fid_last_diamonds")
+        counts = np.zeros(max(nf.value, 1), np.int32)
+        _lib.check(self.lib.fid_last_diamonds(self.h, 0, C.byref(nf), counts.ctypes.data_as(C.c_void_p), None), "fid_last_diamonds")
+        m = max(int(counts.max()), 1)
+        out = (_lib.fid_diamond * (max(nf.value, 1) * m))()
+        _lib.check(self.lib.fid_last_diamonds(self.h, m, C.byref(nf), None, C.cast(out, C.c_void_p)), "fid_last_diamonds")
+        return [self._diamond_split([out[f * m + k] for k in range(int(counts[f]))]) for f in range(nf.value)]
+
     def debug_rejected(self):
         """fid_debug_rejected: detectMarkers' rejectedImgPoints [m, 4, 2] for the last detect() call."""
         n = C.c_int(0)
@@ -384,7 +426,7 @@ class FiducialsNode:
 
     def __init__(self, dictionary=7, fiducial_len=0.14, ignore_fiducials: Iterable[int] = (), fiducial_len_override: Optional[Dict[int, float]] = None,
                  do_pose_estimation=True, device=0, max_width=1920, max_height=1080, max_batch=1, doCornerRefinement=True, cornerRefinementSubPix=True, pose_hypotheses=False,
-                 boards=(), charuco_boards=(), refine_markers=None, **detector_params):
+                 boards=(), charuco_boards=(), refine_markers=None, diamonds=None, **detector_params):
         # doCornerRefinement / cornerRefinementSubPix -> cornerRefinementMethod NONE / SUBPIX / CONTOUR (:700-711, configCallback :274-281)
         if refine_markers is not None and not boards and not charuco_boards:
             raise ValueError("refine_markers needs boards or charuco_boards")
@@ -417,6 +459,11 @@ class FiducialsNode:
         if self.refineMarkers:
             self.det.set_marker_refinement(*refine_markers)
             self.det.set_batch_marker_refinement(True)
+        # ChArUco diamonds (new, no reference counterpart): diamonds = (square_length, marker_length) finds cv2's detectDiamonds among
+        # the markers; the pose results carry `diamonds` = (ids [k, 4], corners [k, 4, 2], fid_diamond records with the poses)
+        self.diamondGeometry = diamonds
+        if diamonds is not None:
+            self.det.set_diamonds(*diamonds)
         self._recovered = []
         self._last_frame = None  # the frame of the last imageCallback, for the ChArUco corners of poseEstimateCallback
         self.haveCamInfo = False
@@ -459,7 +506,7 @@ class FiducialsNode:
                 self.ids, self.corners = self.det.detect(bgr)  # :350
         except _lib.FidError:
             return None  # frame dropped (:389-394)
-        if self.charucoBoards:
+        if self.charucoBoards or self.diamondGeometry is not None:
             self._last_frame = np.ascontiguousarray(bgr, np.uint8)
         for i, fid in enumerate(self.ids.tolist()):
             if fid in self.ignoreIds:
@@ -490,6 +537,7 @@ class FiducialsNode:
             hyps = self.det.pose_hypotheses(self.ids, self.corners, self.K, self.D, self.fiducial_len, self.fiducialLens) if self.poseHypotheses else None
             boards = self.det.board_poses(self.ids, self.corners, self.K, self.D) if self.boards else None
             charuco = self.det.charuco(self._last_frame, self.ids, self.corners, self.K, self.D) if self.charucoBoards and self._last_frame is not None else None
+            diamonds = self.det.diamonds(self._last_frame, self.ids, self.corners, self.K, self.D) if self.diamondGeometry is not None and self._last_frame is not None else None
         except _lib.FidError:
             return fta
         if self.vis_msgs:  # :403, :462-478: vision_msgs/Detection2DArray instead of FiducialTransformArray
@@ -504,6 +552,8 @@ class FiducialsNode:
                 vma.board_poses = boards
             if charuco is not None:
                 vma.charuco = charuco
+            if diamonds is not None:
+                vma.diamonds = diamonds
             if self.refineMarkers:
                 vma.recovered = self._recovered
             return vma
@@ -517,6 +567,8 @@ class FiducialsNode:
             fta.board_poses = boards
         if charuco is not None:
             fta.charuco = charuco
+        if diamonds is not None:
+            fta.diamonds = diamonds
         if self.refineMarkers:
             fta.recovered = self._recovered
         return fta
@@ -533,6 +585,7 @@ class FiducialsNode:
         boards = self.det.last_board_poses() if self.boards else None
         charuco = self.det.last_charuco() if self.charucoBoards else None
         refined = self.det.last_marker_refinement() if self.refineMarkers else None
+        diamonds = self.det.last_diamonds() if self.diamondGeometry is not None else None
         out = []
         for f in range(len(counts)):
             fta = FiducialTransformArray(header=Header(0, (0, 0), self.frameId), image_seq=first_seq + f)
@@ -546,6 +599,8 @@ class FiducialsNode:
                 fta.board_poses = boards[f]
             if charuco is not None:
                 fta.charuco = charuco[f]
+            if diamonds is not None:
+                fta.diamonds = diamonds[f]
             if refined is not None:
                 fta.recovered = self._recovered_of(ids[f, : int(counts[f])], refined[f][0], refined[f][1])
             out.append(fta)

@@ -300,6 +300,46 @@ int fid_refine_detected_markers(fid_detector* h, const uint8_t* bgr, int width, 
                                 int max_markers, int n_rejected, const float* rejected, const fid_camera* cam, int* n_out, int32_t* recovered_idx,
                                 int32_t* recovered_board);
 
+/* ChArUco diamonds (NEW): a 3x3 chessboard with four markers around the centre square, named by the four marker ids, as
+ * cv::aruco::CharucoDetector(CharucoBoard((3, 3), square_length, marker_length, dictionary)).detectDiamonds(image, diamondCorners,
+ * diamondIds, markerCorners, markerIds) of OpenCV 4.13 finds them among markers it is given.  Each marker in list order that is not
+ * part of a diamond yet tries to become the top marker of one: refineDetectedMarkers against a temporary diamond with the ids
+ * {id, id + 2, id + 3, id + 4} and no camera looks for the other three among the remaining markers (within 1.302455 times the root
+ * of the sum of the marker's squared sides; with CORNER_REFINE_SUBPIX the markers it takes get cornerSubPix, and cv2 keeps that
+ * change in its marker list, as this library does internally); when all three are found, detectBoard on the temporary board (the
+ * detector's camera if set, otherwise local homographies; min_markers, check_markers) gives the four chessboard corners.  A diamond
+ * is reported when all four survive, in the order found, its corners in cv2's order (0, 1, 3, 2 of the board's corner ids).  With a
+ * camera its pose is cv::solvePnP(SOLVEPNP_ITERATIVE) of the corners on getSingleMarkerObjectPoints(square_length), packed as every
+ * fid_transform (fid_pose's arithmetic, square_length as the marker length). */
+#define FID_MAX_DIAMONDS (FID_MAX_MARKERS / 4) /* per frame: every diamond takes four markers */
+typedef struct fid_diamond_params {
+    int32_t enable;                /* 0 = off (the default) */
+    float square_length, marker_length;  /* metres, 0 < marker_length < square_length */
+    int32_t min_markers;           /* CharucoParameters::minMarkers, 0..2 (cv2 default 2) */
+    int32_t check_markers;         /* CharucoParameters::checkMarkers (cv2 default 1) */
+} fid_diamond_params;
+typedef struct fid_diamond {
+    int32_t ids[4];                /* cv2's diamondIds: the top marker, then the ones found at the left, right and bottom */
+    float corners[8];              /* x0, y0 .. x3, y3 */
+    int32_t status;                /* 1 pose, 0 no camera */
+    fid_transform pose;            /* fiducial_id = ids[0] */
+} fid_diamond;
+/* Set the diamond geometry of the handle (one per handle, as one cv2 CharucoDetector; copied).  With it on, every batch
+ * (fid_detect_pose_batch, fid_submit_batch) also finds the diamonds of each frame on the device after every other stage, from the
+ * frame's final markers (those recovered by batch refinement included), with the batch's camera; without a camera there is no pose.
+ * fid_detect stays detectMarkers alone.  With it off the batch calls launch exactly what they launch otherwise.  The first enable
+ * allocates the buffers.  FID_ERR_INVALID_ARG for non-finite or out-of-range values, or while batches are in flight. */
+int fid_set_diamonds(fid_detector* h, const fid_diamond_params* params);
+/* The diamonds of one frame (in the fid_set_input_encoding format) and markers already detected (0 <= n <= FID_MAX_MARKERS; ids /
+ * corners as fid_detect returns them; they are not changed): *n_diamonds records in out, which has room for n / 4.  cam may be
+ * NULL.  FID_ERR_INVALID_ARG if diamonds are off or while batches are in flight. */
+int fid_detect_diamonds(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int n, const int32_t* ids, const float* corners,
+                        const fid_camera* cam, int* n_diamonds, fid_diamond* out);
+/* The diamonds of the batch most recently returned by fid_collect_batch / fid_detect_pose_batch: counts[f] and out dense
+ * [n_frames][max_diamonds].  *n_frames = that batch's frame count; counts and out may be NULL to query it.  FID_ERR_INVALID_ARG if
+ * that batch ran without diamonds; FID_ERR_CAPACITY, with nothing written, if a frame has more than max_diamonds. */
+int fid_last_diamonds(fid_detector* h, int max_diamonds, int* n_frames, int32_t* counts, fid_diamond* out);
+
 /* Pixel format of the frames handed to every entry point that takes `bgr` (default FID_ENC_BGR8).  The
  * reference converts whatever the camera publishes with cv_bridge::toCvCopy(msg, BGR8)
  * (aruco_detect.cpp:348) before detectMarkers turns it into gray again; the library takes the camera's own
