@@ -170,6 +170,22 @@ class fid_diamond(C.Structure):
 FID_MAX_DIAMONDS = 64
 
 
+class fid_calib_criteria(C.Structure):
+    _fields_ = [("type", C.c_int32), ("max_iter", C.c_int32), ("epsilon", C.c_double)]
+
+
+class fid_calib_result(C.Structure):
+    _fields_ = [("rms", C.c_double), ("camera", fid_camera), ("std_intrinsics", C.c_double * 9), ("iterations", C.c_int32), ("status", C.c_int32)]
+
+
+FID_CALIB_MAX_STEPS = 2048
+
+
+class fid_calib_stats(C.Structure):
+    _fields_ = [("n_steps", C.c_int32), ("n_evaluations", C.c_int32), ("kernel_launches", C.c_int32), ("reserved", C.c_int32), ("device_ms", C.c_double),
+                ("steps", C.c_uint8 * FID_CALIB_MAX_STEPS)]
+
+
 class fid_map_params(C.Structure):
     _fields_ = [
         ("weighting_scale", C.c_double),
@@ -216,7 +232,7 @@ EXPORTS = [
     "fid_debug_candidates", "fid_debug_rejected", "fid_last_stage_ms", "fid_last_counters", "fid_map_default_params", "fid_map_create", "fid_map_destroy", "fid_map_clear",
     "fid_map_load", "fid_map_links", "fid_map_add_links", "fid_map_update", "fid_map_update_sequence", "fid_map_update_frames", "fid_map_update_frames_async", "fid_map_sync", "fid_map_entries", "fid_map_export", "fid_map_merge", "fid_map_export_device",
     "fid_map_merge_device", "fid_map_merge_device_async", "fid_map_export_async", "fid_map_stream", "fid_map_merged_entries", "fid_map_adopt_merged", "fid_map_add_fiducial", "fid_map_refine_default_params", "fid_map_refine",
-    "fid_jpeg_create", "fid_jpeg_destroy", "fid_jpeg_decode_batch", "fid_jpeg_sync", "fid_jpeg_stream", "fid_jpeg_last_stats",
+    "fid_jpeg_create", "fid_jpeg_destroy", "fid_jpeg_decode_batch", "fid_jpeg_sync", "fid_jpeg_stream", "fid_jpeg_last_stats", "fid_calibrate_camera",
 ]
 
 _lib = None
@@ -305,6 +321,8 @@ def load():
     lib.fid_jpeg_sync.argtypes = [vp]
     lib.fid_jpeg_stream.argtypes = [vp, C.POINTER(vp)]
     lib.fid_jpeg_last_stats.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]
+    lib.fid_calibrate_camera.argtypes = [i32, i32, vp, vp, vp, i32, i32, C.POINTER(fid_camera), i32, C.POINTER(fid_calib_criteria), C.POINTER(fid_calib_result), vp, vp,
+                                         vp, vp, C.POINTER(fid_calib_stats)]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError if the build lost a symbol
     _lib = lib

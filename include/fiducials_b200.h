@@ -546,6 +546,64 @@ int fid_map_merged_entries(fid_map* m, int max_entries, int* n, fid_map_entry* e
 int fid_map_adopt_merged(fid_map* m, int instance);
 
 /* ------------------------------------------------------------------------------------------------
+ * Camera calibration.  Replaces cv::calibrateCameraExtended (OpenCV 4.13, calib3d/src/calibration.cpp) for the camera model of
+ * fid_camera (K and k1 k2 p1 p2 k3): the initial intrinsics of cvInitIntrinsicParams2D (planar rigs) or the caller's guess, one
+ * findExtrinsicCameraParams2 per view, then the joint Levenberg-Marquardt of cv2's CvLevMarq schedule, every view's step solved
+ * on the device through the Schur complement of the 9 intrinsics.  Standalone: no detector handle; the device buffers and the
+ * stream are the call's own and are released before it returns.
+ * ---------------------------------------------------------------------------------------------- */
+#define FID_CALIB_USE_INTRINSIC_GUESS 0x00001 /* the flag values are cv2's CALIB_* */
+#define FID_CALIB_FIX_ASPECT_RATIO 0x00002
+#define FID_CALIB_FIX_PRINCIPAL_POINT 0x00004
+#define FID_CALIB_ZERO_TANGENT_DIST 0x00008
+#define FID_CALIB_FIX_FOCAL_LENGTH 0x00010
+#define FID_CALIB_FIX_K1 0x00020
+#define FID_CALIB_FIX_K2 0x00040
+#define FID_CALIB_FIX_K3 0x00080
+#define FID_CALIB_MAX_VIEWS 65536
+#define FID_CALIB_MAX_POINTS 4096       /* per view */
+#define FID_CALIB_MAX_TOTAL (1 << 24)   /* points over all views */
+#define FID_CALIB_MAX_STEPS 2048        /* recorded trial steps (a run takes at most 2 max_iter + 20) */
+/* fid_calib_result.status: why the call returned FID_ERR_INVALID_ARG where cv2 raises */
+#define FID_CALIB_OK 0
+#define FID_CALIB_E_POINTS 1     /* a view with fewer than 4 points (or more than FID_CALIB_MAX_POINTS) */
+#define FID_CALIB_E_NONPLANAR 2  /* no intrinsic guess and an object z off 0 (mean or standard deviation above 1e-5) */
+#define FID_CALIB_E_HOMOGRAPHY 3 /* initIntrinsicParams2D: a view's points give no homography (e.g. collinear) */
+#define FID_CALIB_E_GUESS 4      /* the guess: fx, fy <= 0, principal point outside the image, or an aspect ratio outside [0.01, 100] */
+#define FID_CALIB_E_EXTRINSICS 5 /* findExtrinsicCameraParams2 raises: non-planar view with fewer than 6 points, degenerate DLT */
+#define FID_CALIB_E_INPUT 6      /* non-finite points, bad offsets or sizes */
+/* cv::TermCriteria: type bit 1 = COUNT (max_iter, clamped to 1..1000; else 30), bit 2 = EPS (epsilon; else DBL_EPSILON) */
+typedef struct fid_calib_criteria {
+    int32_t type;
+    int32_t max_iter;
+    double epsilon;
+} fid_calib_criteria;
+typedef struct fid_calib_result {
+    double rms;                   /* cv2's return value */
+    fid_camera camera;            /* cameraMatrix, distCoeffs */
+    double std_intrinsics[9];     /* stdDeviationsIntrinsics[0..8] = fx fy cx cy k1 k2 p1 p2 k3 (cv2's entries 9..17 are 0) */
+    int32_t iterations;           /* CvLevMarq iterations */
+    int32_t status;               /* FID_CALIB_* */
+} fid_calib_result;
+typedef struct fid_calib_stats {
+    int32_t n_steps;              /* trial steps taken */
+    int32_t n_evaluations;        /* Jacobian evaluations (the final one for the standard deviations included) */
+    int32_t kernel_launches;
+    int32_t reserved;
+    double device_ms;             /* CUDA events around the device work */
+    uint8_t steps[FID_CALIB_MAX_STEPS]; /* per trial step: 1 kept, 0 rejected (raised lambda) */
+} fid_calib_stats;
+/* n_views views, view v = points offsets[v] .. offsets[v+1] (offsets[0] = 0) of obj [.][3] and img [.][2] (float32, host).  guess:
+ * K and D for FID_CALIB_USE_INTRINSIC_GUESS, and the aspect ratio K[0] / K[4] for FID_CALIB_FIX_ASPECT_RATIO (NULL = identity K,
+ * zero D).  criteria NULL = cv2's default (COUNT + EPS, 30, DBL_EPSILON).  Outputs (host, optional but result): rvecs, tvecs
+ * [n_views][3], std_extrinsics [n_views][6] (rvec then tvec), per_view_errors [n_views].  FID_ERR_UNSUPPORTED for any other
+ * flag (rational, thin-prism, tilted models, FIX_K4 and up, ...); FID_ERR_INVALID_ARG with result->status where cv2 raises or the
+ * caps above are exceeded; FID_ERR_NO_DEVICE without a usable device. */
+int fid_calibrate_camera(int device, int n_views, const int32_t* offsets, const float* obj, const float* img, int width, int height, const fid_camera* guess,
+                         int32_t flags, const fid_calib_criteria* criteria, fid_calib_result* result, double* rvecs, double* tvecs, double* std_extrinsics,
+                         double* per_view_errors, fid_calib_stats* stats /* optional */);
+
+/* ------------------------------------------------------------------------------------------------
  * JPEG ingest (NEW; SURVEY 8f-1).  Replaces the cv::imdecode that compressed_image_transport runs in front of
  * FiducialsNode::imageCallback (aruco_detect.cpp:332,348; default transport `compressed`,
  * aruco_detect/launch/aruco_detect.launch:6,28).  The Huffman bit stream of every image is decoded on host threads
