@@ -70,6 +70,11 @@ struct Slot {
     int32_t* d_mr_board = nullptr;                     // [max_batch][max_markers]
     int32_t* d_dia_n = nullptr;                        // fid_set_diamonds: [max_batch], allocated by the first enable
     fid_diamond* d_dia = nullptr;                      // [max_batch][FID_MAX_DIAMONDS]
+    // fid_set_dictionaries: allocated when the handle enters multi-dictionary mode
+    int32_t* d_md_count = nullptr;                     // [n_dicts][max_batch]             k_finish per dictionary
+    int32_t* d_md_ids = nullptr;                       // [n_dicts][max_batch][max_markers]
+    float* d_md_corners = nullptr;                     // [n_dicts][max_batch][max_markers][8]
+    int32_t* d_out_dict = nullptr;                     // [max_batch][max_markers]          k_dict_merge
     // pinned host mirrors
     int32_t* h_out_count = nullptr;
     int32_t* h_out_ids = nullptr;
@@ -88,6 +93,7 @@ struct Slot {
     int32_t* h_mr_board = nullptr;
     int32_t* h_dia_n = nullptr;
     fid_diamond* h_dia = nullptr;
+    int32_t* h_out_dict = nullptr;
     Counters* h_counters = nullptr;
     int* h_nsel = nullptr;
     int* h_nrawc = nullptr;
@@ -117,7 +123,7 @@ struct fid_detector {
     struct Pending {
         int first_slot, n_chunks, n_frames, w, h;
         int64_t launches;
-        bool pose, hyp, board, charuco, refine, diamonds;
+        bool pose, hyp, board, charuco, refine, diamonds, multi;
     } pending[MAX_SLOTS]{};
     int pend_head = 0, pend_count = 0, slots_in_use = 0, slot_next = 0;
     cudaStream_t slot_stream[MAX_SLOTS] = {};
@@ -194,6 +200,16 @@ struct fid_detector {
     int last_dia_frames = 0;
     std::vector<int32_t> last_dia_n;                 // [last_dia_frames]
     std::vector<fid_diamond> last_dia;               // frame after frame, last_dia_n[f] each
+    // several dictionaries (fid_set_dictionaries / fid_detect_multi_dict / fid_last_dict_indices)
+    int n_dicts = 1;
+    fid_dictionary_spec dict_spec[FID_MAX_DICTIONARIES]{};  // entry 0's dictionary is params.dictionary
+    DevParams dict_P[FID_MAX_DICTIONARIES]{};        // params with each entry's dictionary
+    bool multi = false;                              // more than one entry, or entry 0 with an offset or a length
+    unsigned long long* d_mdict = nullptr;           // [FID_MAX_DICTIONARIES][kMaxDictMarkers * 4], multi-dictionary mode only
+    bool last_di_valid = false;                      // fid_last_dict_indices
+    int last_di_frames = 0, last_di_stride = 0;
+    std::vector<int32_t> last_di_counts, last_di;    // [last_di_frames][last_di_stride]
+    bool detected_multi = false;                     // slot 0 holds fid_detect_multi_dict's candidates, not detectMarkers'
     int32_t* d_dbg_rej_n = nullptr;                  // fid_debug_rejected: count, then [max_sel][8] floats
     float* d_dbg_rej = nullptr;
     float stage_ms[ST_COUNT + N_WALK_ROUNDS]{};
@@ -382,11 +398,12 @@ static void free_slot(Slot& s) {
                      s.fs.group_members, s.fs.next_in_group, s.fs.group_head, s.fs.group_tail, s.fs.close_count, s.fs.close_idx,   s.fs.close_off,  s.fs.selected,
                      s.fs.sel_idx,    s.d_nsel,          s.d_nrawc,         s.d_cand_id,      s.d_cand_corners, s.d_out_count,    s.d_out_ids,     s.d_out_corners,
                      s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp, s.d_out_board, s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy,
-                     s.d_rej_n,       s.d_rej,           s.d_mr_nrec,       s.d_mr_idx,       s.d_mr_board,    s.d_dia_n,       s.d_dia};
+                     s.d_rej_n,       s.d_rej,           s.d_mr_nrec,       s.d_mr_idx,       s.d_mr_board,    s.d_dia_n,       s.d_dia,
+                     s.d_md_count,    s.d_md_ids,        s.d_md_corners,    s.d_out_dict};
     for (void* p : dptrs)
         if (p) cudaFree(p);
     void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp, s.h_out_board, s.h_out_ch, s.h_out_ch_ids, s.h_out_ch_xy,
-                     s.h_rej_n,     s.h_rej,     s.h_mr_nrec,    s.h_mr_idx,   s.h_mr_board, s.h_dia_n, s.h_dia};
+                     s.h_rej_n,     s.h_rej,     s.h_mr_nrec,    s.h_mr_idx,   s.h_mr_board, s.h_dia_n, s.h_dia, s.h_out_dict};
     for (void* p : hptrs)
         if (p) cudaFreeHost(p);
     for (int i = 0; i <= ST_COUNT; i++)
@@ -414,6 +431,8 @@ extern "C" int fid_create(const fid_params* params, int device, int max_width, i
     h->device = device;
     h->params = *params;
     h->P = P;
+    h->dict_spec[0].dictionary = params->dictionary;
+    h->dict_P[0] = P;
     h->max_w = max_width;
     h->max_h = max_height;
     h->max_batch = max_batch;
@@ -539,7 +558,7 @@ extern "C" int fid_destroy(fid_detector* h) {
     void* ptrs[] = {h->d_prune, h->d_dict, h->d_pf[0], h->d_pf[1], h->d_lut_prev, h->d_lut_next, h->d_subpix_masks, h->d_override_ids, h->d_override_lens, h->d_pose_ids, h->d_pose_corners, h->d_pose_out, h->d_hyp_list,
                      h->d_board_off, h->d_board_keys, h->d_board_marker, h->d_board_obj, h->d_board_count, h->d_board_list, h->d_ch_boards, h->d_ch_keys,
                      h->d_ch_marker, h->d_ch_ids, h->d_ch_near_n, h->d_ch_near_idx, h->d_ch_near_corner, h->d_ch_obj, h->d_ch_chess, h->d_ch_masks,
-                     h->d_ch_count, h->d_ch_list, h->d_ch_list_ids, h->d_ch_list_xy, h->d_mr_i, h->d_mr_f, h->d_dbg_rej_n, h->d_dbg_rej, h->d_dia_io, h->d_dia_list};
+                     h->d_ch_count, h->d_ch_list, h->d_ch_list_ids, h->d_ch_list_xy, h->d_mr_i, h->d_mr_f, h->d_dbg_rej_n, h->d_dbg_rej, h->d_dia_io, h->d_dia_list, h->d_mdict};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     for (int i = 0; i < 2; i++)
@@ -554,18 +573,86 @@ extern "C" int fid_destroy(fid_detector* h) {
     return FID_OK;
 }
 
+// DevParams of the first n dictionary entries under params p: entry 0 takes p.dictionary, entry d > 0 specs[d].dictionary.
+static int dict_params(const fid_params& p, int n, const fid_dictionary_spec* specs, DevParams* out) {
+    for (int d = 0; d < n; d++) {
+        fid_params q = p;
+        if (d > 0) q.dictionary = specs[d].dictionary;
+        const int rc = make_dev_params(q, &out[d]);
+        if (rc != FID_OK) return rc;
+    }
+    return FID_OK;
+}
+
+// multi-dictionary mode: every entry's table -> device, entry d at d * kMaxDictMarkers * 4 words
+static int upload_dictionaries(fid_detector* h) {
+    std::vector<unsigned long long> words;
+    for (int d = 0; d < h->n_dicts; d++) {
+        pack_dictionary(h->dict_P[d], &words);
+        CK(cudaMemcpy(h->d_mdict + (size_t)d * kMaxDictMarkers * 4, words.data(), words.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice));
+    }
+    return FID_OK;
+}
+
 extern "C" int fid_set_params(fid_detector* h, const fid_params* params) {
     if (!h || !params) return FID_ERR_INVALID_ARG;
     DevParams P;
-    const int rc = make_dev_params(*params, &P);
+    int rc = make_dev_params(*params, &P);
     if (rc != FID_OK) return rc;
     if (h->pend_count) return FID_ERR_INVALID_ARG;  // between frames only (configCallback, aruco_detect.cpp:257-298)
+    DevParams dp[FID_MAX_DICTIONARIES];             // entries 1.. keep their dictionaries under the new parameters (cv2's setDictionary)
+    if (h->n_dicts > 1 && (rc = dict_params(*params, h->n_dicts, h->dict_spec, dp)) != FID_OK) return rc;
+    if ((int64_t)h->dict_spec[0].id_offset + P.n_markers - 1 > INT32_MAX) return FID_ERR_INVALID_ARG;  // entry 0's published ids
     CK(cudaSetDevice(h->device));
     for (int i = 0; i < h->n_slots; i++) CK(cudaStreamSynchronize(h->slot_stream[i]));
     CK(cudaStreamSynchronize(h->stream));
     h->params = *params;
     h->P = P;
-    return upload_dictionary(h);
+    h->dict_spec[0].dictionary = params->dictionary;
+    h->dict_P[0] = P;
+    for (int d = 1; d < h->n_dicts; d++) h->dict_P[d] = dp[d];
+    if ((rc = upload_dictionary(h)) != FID_OK) return rc;
+    return h->multi ? upload_dictionaries(h) : FID_OK;
+}
+
+extern "C" int fid_set_dictionaries(fid_detector* h, int n, const fid_dictionary_spec* specs) {
+    if (!h || !specs || n < 1 || n > FID_MAX_DICTIONARIES || h->pend_count) return FID_ERR_INVALID_ARG;
+    fid_params p = h->params;
+    p.dictionary = specs[0].dictionary;
+    DevParams dp[FID_MAX_DICTIONARIES];
+    int rc = dict_params(p, n, specs, dp);
+    if (rc != FID_OK) return rc;
+    for (int d = 0; d < n; d++) {
+        if (!std::isfinite(specs[d].fiducial_len) || specs[d].fiducial_len < 0) return FID_ERR_INVALID_ARG;
+        if ((int64_t)specs[d].id_offset + dp[d].n_markers - 1 > INT32_MAX) return FID_ERR_INVALID_ARG;  // a published id would overflow
+    }
+    const bool multi = n > 1 || specs[0].id_offset != 0 || specs[0].fiducial_len > 0;
+    if (multi && (h->n_boards || h->n_charuco || h->batch_refine || h->diamond.enable)) return FID_ERR_UNSUPPORTED;
+    CK(cudaSetDevice(h->device));
+    if (multi) {  // (a failed allocation leaves the handle as it was; the next call completes it)
+        const size_t F = h->max_batch, M = F * h->max_markers, ND = FID_MAX_DICTIONARIES;
+        if (!h->d_mdict && (rc = dalloc(&h->d_mdict, ND * kMaxDictMarkers * 4)) != FID_OK) return rc;
+        for (int i = 0; i < h->n_slots; i++) {
+            Slot& s = h->slot[i];
+            if (!s.d_md_count && (rc = dalloc(&s.d_md_count, ND * F)) != FID_OK) return rc;
+            if (!s.d_md_ids && (rc = dalloc(&s.d_md_ids, ND * M)) != FID_OK) return rc;
+            if (!s.d_md_corners && (rc = dalloc(&s.d_md_corners, ND * M * 8)) != FID_OK) return rc;
+            if (!s.d_out_dict && (rc = dalloc(&s.d_out_dict, M)) != FID_OK) return rc;
+            if (!s.h_out_dict && (rc = halloc(&s.h_out_dict, M)) != FID_OK) return rc;
+        }
+    }
+    for (int i = 0; i < h->n_slots; i++) CK(cudaStreamSynchronize(h->slot_stream[i]));
+    CK(cudaStreamSynchronize(h->stream));
+    h->params = p;
+    h->P = dp[0];
+    h->n_dicts = n;
+    h->multi = multi;
+    for (int d = 0; d < n; d++) {
+        h->dict_spec[d] = specs[d];
+        h->dict_P[d] = dp[d];
+    }
+    if ((rc = upload_dictionary(h)) != FID_OK) return rc;
+    return multi ? upload_dictionaries(h) : FID_OK;
 }
 
 static Camera make_camera(const fid_camera* c) {
@@ -722,7 +809,8 @@ static DiamondArgs diamond_args(const fid_detector* h, const uint8_t* src, size_
 static bool batch_refines(const fid_detector* h) { return h->batch_refine && h->mrefine.enable && h->n_boards + h->n_charuco > 0; }
 
 static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, const FrameGeom& g, const uint8_t* d_bgr, const fid_camera* cam, double fiducial_len,
-                            int n_override, int stop_after /* -1 = all */, const Slot* prev = nullptr, bool refine = false, bool diamonds = false) {
+                            int n_override, int stop_after /* -1 = all */, const Slot* prev = nullptr, bool refine = false, bool diamonds = false,
+                            bool multi = false) {
     const DevParams& P = h->P;
     const int W = g.W, H = g.H;
     int launches = 0;
@@ -902,7 +990,8 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
     }
     CK(cudaEventRecord(s.ev[ST_GROUP], st));
     if (stop_after == ST_APPROX) return FID_OK;
-    {  // sort + group
+    // grouping, identification, CORNER_REFINE_CONTOUR and k_finish for one dictionary's parameters and table
+    auto group = [&](int marker_size) {
         GroupArgs a{};
         a.raw = s.d_raw;
         a.n_raw = s.d_nraw;
@@ -912,7 +1001,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.max_raw = h->max_raw;
         a.close_wpr = h->close_wpr;
         a.max_sel = h->max_sel;
-        a.marker_size = P.marker_size;
+        a.marker_size = marker_size;
         a.border_bits = P.marker_border_bits;
         a.min_marker_dist_rate = (float)P.min_marker_dist_rate;
         a.min_group_dist = (float)P.min_group_dist;
@@ -925,9 +1014,8 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.prof = group_prof;
         launch_prio(k_sort_group, dim3(nf), dim3(GROUP_THREADS), group_smem(h->max_raw), st, 4, a);
         launches++;
-    }
-    CK(cudaEventRecord(s.ev[ST_IDENT], st));
-    {  // identify
+    };
+    auto identify = [&](const DevParams& Pd, const unsigned long long* dict) {
         IdentifyArgs a{};
         a.src = d_bgr;
         a.row_stride = g.bgr_row_stride;
@@ -939,8 +1027,8 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.n_sel = s.d_nsel;
         a.max_raw = h->max_raw;
         a.max_sel = h->max_sel;
-        a.P = P;
-        a.dict = h->d_dict;
+        a.P = Pd;
+        a.dict = dict;
         a.cand_id = s.d_cand_id;
         a.cand_corners = s.d_cand_corners;
         a.cand_raw = s.d_cand_raw;
@@ -948,12 +1036,11 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.retry_list = s.d_retry_list;
         a.counters = s.d_counters;
         // fixed grids over work lists: a grid of one block per (frame, candidate slot) is 32 768 blocks of which 1 500 have work
-        launch_prio(k_identify_first, dim3(h->sm_count * 4), dim3(IDENT0_WARPS * 32), ident_smem(P, IDENT0_WARPS), st, 4, a);
-        launch_prio(k_identify_retry, dim3(h->sm_count * 2), dim3(IDENT_WARPS * 32), ident_smem(P, IDENT_WARPS), st, 4, a);
+        launch_prio(k_identify_first, dim3(h->sm_count * 4), dim3(IDENT0_WARPS * 32), ident_smem(Pd, IDENT0_WARPS), st, 4, a);
+        launch_prio(k_identify_retry, dim3(h->sm_count * 2), dim3(IDENT_WARPS * 32), ident_smem(Pd, IDENT_WARPS), st, 4, a);
         launches += 2;
-    }
-    CK(cudaEventRecord(s.ev[ST_SUBPIX_POSE], st));
-    if (P.corner_refine == 2) {  // CORNER_REFINE_CONTOUR: rewrite the decoded candidates' corners before the output stage
+    };
+    auto contour_refine = [&]() {  // CORNER_REFINE_CONTOUR: rewrite the decoded candidates' corners before the output stage
         ContourRefineArgs a{};
         a.n_sel = s.d_nsel;
         a.cand_id = s.d_cand_id;
@@ -965,8 +1052,8 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.max_sel = h->max_sel;
         launch_prio(k_contour_refine, dim3(h->max_sel, nf), dim3(CREFINE_THREADS), 0, st, 5, a);
         launches++;
-    }
-    {  // finish
+    };
+    auto finish = [&](const DevParams& Pd, const fid_camera* fcam, int32_t* out_count, int32_t* out_ids, float* out_corners) {
         FinishArgs a{};
         a.src = d_bgr;
         a.row_stride = g.bgr_row_stride;
@@ -981,22 +1068,77 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.max_raw = h->max_raw;
         a.max_sel = h->max_sel;
         a.max_markers = h->max_markers;
-        a.P = P;
+        a.P = Pd;
         a.subpix_masks = h->d_subpix_masks;
+        a.do_pose = fcam ? 1 : 0;
+        a.cam = make_camera(fcam);
+        a.fiducial_len = fiducial_len;
+        a.n_override = n_override;
+        a.override_ids = h->d_override_ids;
+        a.override_lens = h->d_override_lens;
+        a.out_count = out_count;
+        a.out_ids = out_ids;
+        a.out_corners = out_corners;
+        a.out_tf = s.d_out_tf;
+        a.counters = s.d_counters;
+        launch_prio(k_finish, dim3(nf), dim3(FINISH_THREADS), 0, st, 5, a);
+        launches++;
+    };
+    if (multi) {  // several dictionaries (fid_set_dictionaries): the front end above ran once
+        const size_t F = h->max_batch, dstride = F * h->max_markers;
+        int grouped = -1;
+        for (int d = 0; d < h->n_dicts; d++) {
+            const DevParams& Pd = h->dict_P[d];
+            if (Pd.marker_size != grouped) {  // filterTooCloseCandidates depends on the marker size only
+                CK(cudaMemsetAsync(&s.d_counters->n_first, 0, sizeof(unsigned int), st));
+                group(Pd.marker_size);
+                grouped = Pd.marker_size;
+            }
+            CK(cudaMemsetAsync(&s.d_counters->n_retry, 0, sizeof(unsigned int), st));
+            identify(Pd, h->d_mdict + (size_t)d * kMaxDictMarkers * 4);
+            if (Pd.corner_refine == 2) contour_refine();
+            finish(Pd, nullptr, s.d_md_count + d * F, s.d_md_ids + d * dstride, s.d_md_corners + d * dstride * 8);
+        }
+        // the stages interleave per dictionary: ST_GROUP holds all of them, ST_IDENT is empty, ST_SUBPIX_POSE is the merge
+        CK(cudaEventRecord(s.ev[ST_IDENT], st));
+        CK(cudaEventRecord(s.ev[ST_SUBPIX_POSE], st));
+        DictMergeArgs a{};
+        a.n_dicts = h->n_dicts;
+        a.dict_stride = dstride;
+        a.count = s.d_md_count;
+        a.ids = s.d_md_ids;
+        a.corners = s.d_md_corners;
+        a.F = (int)F;
+        a.max_markers = h->max_markers;
+        for (int d = 0; d < h->n_dicts; d++) {
+            a.dp[d].id_offset = h->dict_spec[d].id_offset;
+            a.dp[d].len = h->dict_spec[d].fiducial_len > 0 ? h->dict_spec[d].fiducial_len : fiducial_len;
+        }
         a.do_pose = cam ? 1 : 0;
         a.cam = make_camera(cam);
-        a.fiducial_len = fiducial_len;
         a.n_override = n_override;
         a.override_ids = h->d_override_ids;
         a.override_lens = h->d_override_lens;
         a.out_count = s.d_out_count;
         a.out_ids = s.d_out_ids;
         a.out_corners = s.d_out_corners;
+        a.out_dict = s.d_out_dict;
         a.out_tf = s.d_out_tf;
+        a.out_hyp = (h->pose_hyp && cam) ? s.d_out_hyp : nullptr;
         a.counters = s.d_counters;
-        launch_prio(k_finish, dim3(nf), dim3(FINISH_THREADS), 0, st, 5, a);
+        launch_prio(k_dict_merge, dim3(nf), dim3(DICT_MERGE_THREADS), 0, st, 5, a);
         launches++;
+        CK(cudaEventRecord(s.ev[ST_D2H], st));
+        h->counters[6] += launches;
+        CK(cudaGetLastError());
+        return FID_OK;
     }
+    group(P.marker_size);
+    CK(cudaEventRecord(s.ev[ST_IDENT], st));
+    identify(P, h->d_dict);
+    CK(cudaEventRecord(s.ev[ST_SUBPIX_POSE], st));
+    if (P.corner_refine == 2) contour_refine();
+    finish(P, cam, s.d_out_count, s.d_out_ids, s.d_out_corners);
     if (refine) {  // opt-in: recover missed board markers before the stages that read the markers (fid_set_batch_marker_refinement)
         RejectedArgs ra{};
         ra.n_sel = s.d_nsel;
@@ -1083,8 +1225,9 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
 }
 
 static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose, bool with_hyp, bool with_board, bool with_charuco, bool with_refine,
-                       bool with_diamonds) {
+                       bool with_diamonds, bool multi = false) {
     const size_t M = (size_t)nf * h->max_markers;
+    if (multi) CK(cudaMemcpyAsync(s.h_out_dict, s.d_out_dict, sizeof(int32_t) * M, cudaMemcpyDeviceToHost, st));
     if (with_diamonds) CK(cudaMemcpyAsync(s.h_dia_n, s.d_dia_n, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));  // collect copies the records
     if (with_refine) {  // counts only: collect copies the lists at their lengths
         CK(cudaMemcpyAsync(s.h_rej_n, s.d_rej_n, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));
@@ -1110,7 +1253,8 @@ static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool w
 }
 
 static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* tfs, bool first_chunk,
-                   struct fid_pose_hypotheses* hyps = nullptr, fid_board_pose* boards = nullptr, int ch_first = -1, bool refined = false, bool diamonds = false) {
+                   struct fid_pose_hypotheses* hyps = nullptr, fid_board_pose* boards = nullptr, int ch_first = -1, bool refined = false, bool diamonds = false,
+                   int32_t* dict_idx = nullptr, bool multi = false) {
     CK(cudaEventSynchronize(s.done));
     int status = FID_OK;
     if (diamonds) {  // the diamond records (fid_last_diamonds), each row at the frame with the most diamonds
@@ -1161,6 +1305,8 @@ static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* c
         if (corners) memcpy(corners + (size_t)f * max_markers * 8, s.h_out_corners + (size_t)f * h->max_markers * 8, sizeof(float) * 8 * n);
         if (tfs) memcpy(tfs + (size_t)f * max_markers, s.h_out_tf + (size_t)f * h->max_markers, sizeof(fid_transform) * n);
         if (hyps) memcpy(hyps + (size_t)f * max_markers, s.h_out_hyp + (size_t)f * h->max_markers, sizeof(struct fid_pose_hypotheses) * n);
+        if (dict_idx && multi) memcpy(dict_idx + (size_t)f * max_markers, s.h_out_dict + (size_t)f * h->max_markers, sizeof(int32_t) * n);
+        if (dict_idx && !multi) memset(dict_idx + (size_t)f * max_markers, 0, sizeof(int32_t) * n);
     }
     if (boards) memcpy(boards, s.h_out_board, sizeof(fid_board_pose) * nf * h->n_boards);
     if (ch_first >= 0) {  // frames ch_first .. of the ChArUco records of the batch (fid_last_charuco)
@@ -1226,6 +1372,19 @@ static void end_last_hypotheses(fid_detector* h, bool hyp, const int32_t* counts
     h->last_hyp_valid = true;
 }
 
+// The same for the dictionary indices (fid_last_dict_indices), kept for every batch.
+static int32_t* begin_last_dict_indices(fid_detector* h, int n_frames, int max_markers) {
+    h->last_di_valid = false;
+    h->last_di_frames = n_frames;
+    h->last_di_stride = max_markers;
+    h->last_di.resize((size_t)n_frames * max_markers);
+    return h->last_di.data();
+}
+static void end_last_dict_indices(fid_detector* h, const int32_t* counts) {
+    h->last_di_counts.assign(counts, counts + h->last_di_frames);
+    h->last_di_valid = true;
+}
+
 // The same for the board poses (fid_last_board_poses), dense [n_frames][n_boards].
 static fid_board_pose* begin_last_boards(fid_detector* h, bool board, int n_frames) {
     h->last_board_valid = false;
@@ -1272,7 +1431,7 @@ static void begin_last_diamonds(fid_detector* h, bool dia, int n_frames) {
 // fid_detect_pose_batch; fid_detect (detectMarkers) passes may_refine = false, which also leaves diamonds out.
 static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
                              const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
-                             int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms, bool may_refine) {
+                             int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms, bool may_refine, bool multi) {
     if (!h || !bgr || !counts || n_frames < 0 || width < 16 || height < 16 || width > h->max_w || height > h->max_h || max_markers < 0) return FID_ERR_INVALID_ARG;
     if (row_stride < (size_t)width * h->bpp || frame_stride < row_stride * (size_t)height) return FID_ERR_INVALID_ARG;
     if (cam && !(fiducial_len > 0)) return FID_ERR_INVALID_ARG;
@@ -1295,6 +1454,7 @@ static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, 
     begin_last_refinement(h, mr, n_frames);
     const bool dia = may_refine && h->diamond.enable;
     begin_last_diamonds(h, dia, n_frames);
+    int32_t* dict_idx = begin_last_dict_indices(h, n_frames, max_markers);
     h->counters[6] = 0;
     h->stage_ms[ST_H2D] = 0;
     // software pipeline over chunks: up to n_slots chunks in flight, each on its own stream; results of
@@ -1345,9 +1505,9 @@ static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, 
                 h->pf_h = height;
                 h->hint_next = nullptr;
             }
-            rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, c > 0 ? &h->slot[(c - 1) % NS] : nullptr, mr, dia);
+            rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, c > 0 ? &h->slot[(c - 1) % NS] : nullptr, mr, dia, multi);
             if (rc != FID_OK) return rc;
-            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp, brd, chr, mr, dia);
+            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp, brd, chr, mr, dia, multi);
             if (rc != FID_OK) return rc;
             h->last_frames = nf;
         }
@@ -1357,11 +1517,13 @@ static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, 
             const int nf = std::min(B, n_frames - pc * B);
             rc = collect(h, s, nf, max_markers, counts + (size_t)pc * B, ids ? ids + (size_t)pc * B * max_markers : nullptr,
                          corners ? corners + (size_t)pc * B * max_markers * 8 : nullptr, (transforms && cam) ? transforms + (size_t)pc * B * max_markers : nullptr, pc == 0,
-                         hyps ? hyps + (size_t)pc * B * max_markers : nullptr, boards ? boards + (size_t)pc * B * h->n_boards : nullptr, chr ? pc * B : -1, mr, dia);
+                         hyps ? hyps + (size_t)pc * B * max_markers : nullptr, boards ? boards + (size_t)pc * B * h->n_boards : nullptr, chr ? pc * B : -1, mr, dia,
+                         dict_idx + (size_t)pc * B * max_markers, multi);
             if (rc != FID_OK) status = rc;
         }
     }
     end_last_hypotheses(h, hyp, counts);
+    end_last_dict_indices(h, counts);
     h->last_board_valid = brd;
     h->last_ch_valid = chr;
     h->last_mr_valid = mr;
@@ -1373,7 +1535,7 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
                                      const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
                                      int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms) {
     return detect_pose_batch(h, n_frames, bgr, bgr_on_device, width, height, row_stride, frame_stride, cam, fiducial_len, n_override, override_ids, override_lens,
-                             max_markers, counts, ids, corners, transforms, true);
+                             max_markers, counts, ids, corners, transforms, true, h && h->multi);
 }
 
 extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
@@ -1421,9 +1583,9 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
             g = make_geom(h, width, height, (size_t)width * h->bpp, (size_t)width * h->bpp * height);
         }
         const Slot* prev = (h->slots_in_use + c) > 0 ? &h->slot[(si + NS - 1) % NS] : nullptr;
-        rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, prev, mr, dia);
+        rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, prev, mr, dia, h->multi);
         if (rc != FID_OK) return rc;
-        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam, h->n_boards && cam, h->n_charuco > 0, mr, dia);
+        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam, h->n_boards && cam, h->n_charuco > 0, mr, dia, h->multi);
         if (rc != FID_OK) return rc;
         h->last_frames = nf;
     }
@@ -1439,6 +1601,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
     pb.charuco = h->n_charuco > 0;
     pb.refine = mr;
     pb.diamonds = dia;
+    pb.multi = h->multi;
     pb.launches = h->counters[6];
     h->pend_count++;
     h->slots_in_use += n_chunks;
@@ -1459,16 +1622,18 @@ extern "C" int fid_collect_batch(fid_detector* h, int max_markers, int32_t* coun
     begin_last_charuco(h, pb.charuco, pb.n_frames);
     begin_last_refinement(h, pb.refine, pb.n_frames);
     begin_last_diamonds(h, pb.diamonds, pb.n_frames);
+    int32_t* dict_idx = begin_last_dict_indices(h, pb.n_frames, max_markers);
     for (int c = 0; c < pb.n_chunks; c++) {
         Slot& s = h->slot[(pb.first_slot + c) % NS];
         const int nf = std::min(B, pb.n_frames - c * B);
         const int rc = collect(h, s, nf, max_markers, counts + (size_t)c * B, ids ? ids + (size_t)c * B * max_markers : nullptr,
                                corners ? corners + (size_t)c * B * max_markers * 8 : nullptr, (transforms && pb.pose) ? transforms + (size_t)c * B * max_markers : nullptr, c == 0,
                                hyps ? hyps + (size_t)c * B * max_markers : nullptr, boards ? boards + (size_t)c * B * h->n_boards : nullptr,
-                               pb.charuco ? c * B : -1, pb.refine, pb.diamonds);
+                               pb.charuco ? c * B : -1, pb.refine, pb.diamonds, dict_idx + (size_t)c * B * max_markers, pb.multi);
         if (rc != FID_OK) status = rc;
     }
     end_last_hypotheses(h, pb.hyp, counts);
+    end_last_dict_indices(h, counts);
     h->last_board_valid = pb.board;
     h->last_ch_valid = pb.charuco;
     h->last_mr_valid = pb.refine;
@@ -1482,10 +1647,40 @@ extern "C" int fid_collect_batch(fid_detector* h, int max_markers, int32_t* coun
 extern "C" int fid_detect(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int max_markers, int* n, int32_t* ids, float* corners) {
     if (!n) return FID_ERR_INVALID_ARG;
     int32_t count = 0;
-    const int rc = detect_pose_batch(h, 1, bgr, 0, width, height, stride, stride * (size_t)height, nullptr, 0.0, 0, nullptr, nullptr, max_markers, &count, ids, corners, nullptr, false);
-    if (rc == FID_OK || rc == FID_ERR_CAPACITY) h->detected = true;
+    const int rc = detect_pose_batch(h, 1, bgr, 0, width, height, stride, stride * (size_t)height, nullptr, 0.0, 0, nullptr, nullptr, max_markers, &count, ids, corners, nullptr, false,
+                                     false);
+    if (rc == FID_OK || rc == FID_ERR_CAPACITY) {
+        h->detected = true;
+        h->detected_multi = false;
+    }
     *n = count;
     return rc;
+}
+
+extern "C" int fid_detect_multi_dict(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int max_markers, int* n, int32_t* ids, float* corners,
+                                     int32_t* dict_indices) {
+    if (!h || !n) return FID_ERR_INVALID_ARG;
+    int32_t count = 0;
+    const int rc = detect_pose_batch(h, 1, bgr, 0, width, height, stride, stride * (size_t)height, nullptr, 0.0, 0, nullptr, nullptr, max_markers, &count, ids, corners, nullptr, false,
+                                     h->multi);
+    if (rc == FID_OK || rc == FID_ERR_CAPACITY) {
+        h->detected = true;
+        h->detected_multi = h->multi;
+        if (dict_indices) memcpy(dict_indices, h->last_di.data(), sizeof(int32_t) * count);
+    }
+    *n = count;
+    return rc;
+}
+
+extern "C" int fid_last_dict_indices(fid_detector* h, int max_markers, int* n_frames, int32_t* out) {
+    if (!h || !n_frames || max_markers < 0 || !h->last_di_valid) return FID_ERR_INVALID_ARG;
+    const int nf = h->last_di_frames;
+    *n_frames = nf;
+    if (!out) return FID_OK;
+    for (int f = 0; f < nf; f++)
+        if (h->last_di_counts[f] > max_markers) return FID_ERR_CAPACITY;
+    for (int f = 0; f < nf; f++) memcpy(out + (size_t)f * max_markers, h->last_di.data() + (size_t)f * h->last_di_stride, sizeof(int32_t) * h->last_di_counts[f]);
+    return FID_OK;
 }
 
 extern "C" int fid_pose(fid_detector* h, int n, const int32_t* ids, const float* corners, const fid_camera* cam, double fiducial_len, int n_override,
@@ -1574,6 +1769,7 @@ extern "C" int fid_last_pose_hypotheses(fid_detector* h, int max_markers, int* n
 extern "C" int fid_set_boards(fid_detector* h, int n_boards, const fid_board* boards) {
     if (!h || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight read the board tables
     if (n_boards < 0 || n_boards > FID_MAX_BOARDS || (n_boards > 0 && !boards)) return FID_ERR_INVALID_ARG;
+    if (n_boards > 0 && h->multi) return FID_ERR_UNSUPPORTED;  // which family a board's ids belong to is not modelled
     std::vector<int32_t> off(1, 0), keys, marker;
     std::vector<float> obj;
     for (int b = 0; b < n_boards; b++) {
@@ -1648,6 +1844,7 @@ extern "C" int fid_last_board_poses(fid_detector* h, int max_boards, int* n_fram
 extern "C" int fid_set_charuco_boards(fid_detector* h, int n_boards, const fid_charuco_board* boards) {
     if (!h || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight read the board tables
     if (n_boards < 0 || n_boards > FID_MAX_CHARUCO_BOARDS || (n_boards > 0 && !boards)) return FID_ERR_INVALID_ARG;
+    if (n_boards > 0 && h->multi) return FID_ERR_UNSUPPORTED;
     std::vector<CharucoBoardDev> bd;
     std::vector<int32_t> keys, marker, ids, near_n, near_idx, near_corner;
     std::vector<float> obj, chess;
@@ -1862,6 +2059,7 @@ extern "C" int fid_refine_detected_markers(fid_detector* h, const uint8_t* bgr, 
 
 extern "C" int fid_set_batch_marker_refinement(fid_detector* h, int enable) {
     if (!h || h->pend_count) return FID_ERR_INVALID_ARG;
+    if (enable && h->multi) return FID_ERR_UNSUPPORTED;
     if (enable) {  // (a failed allocation leaves the option off; the next enable completes it)
         CK(cudaSetDevice(h->device));
         const size_t F = h->max_batch, M = F * h->max_markers;
@@ -1913,6 +2111,7 @@ extern "C" int fid_last_marker_refinement(fid_detector* h, int max_markers, int 
 extern "C" int fid_set_diamonds(fid_detector* h, const fid_diamond_params* params) {
     if (!h || !params || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight read the layout
     const fid_diamond_params p = *params;
+    if (p.enable && h->multi) return FID_ERR_UNSUPPORTED;
     DiamondLayout L{};
     if (p.enable) {
         if (!std::isfinite(p.square_length) || !(p.marker_length > 0) || !(p.marker_length < p.square_length)) return FID_ERR_INVALID_ARG;
@@ -2160,6 +2359,7 @@ extern "C" int fid_debug_candidates(fid_detector* h, int max_candidates, int* n,
 extern "C" int fid_debug_rejected(fid_detector* h, int max_rejected, int* n, float* rejected) {
     if (!h || !n || max_rejected < 0 || h->pend_count) return FID_ERR_INVALID_ARG;
     if (!h->detected) return FID_ERR_INVALID_ARG;  // slot 0's candidate lists were never written
+    if (h->detected_multi) return FID_ERR_UNSUPPORTED;  // detectMarkersMultiDict's rejected list (DESIGN.md finding 15) is not modelled
     CK(cudaSetDevice(h->device));
     int rc;
     if (!h->d_dbg_rej_n && (rc = dalloc(&h->d_dbg_rej_n, 1)) != FID_OK) return rc;

@@ -1553,4 +1553,92 @@ __global__ void __launch_bounds__(DIAMOND_THREADS) k_diamond(const DiamondArgs a
     }
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Several dictionaries (fid_set_dictionaries): k_finish has written each dictionary's markers, without pose, to lists of their
+// own.  k_dict_merge concatenates them in dictionary order (detectMarkersMultiDict), records each marker's dictionary index, and
+// solves the pose of each marker as k_pose does for its published id (id + id_offset) and its dictionary's length; with the
+// pose-hypotheses option also both planar hypotheses, as k_pose_hypotheses.  One block per frame, one thread per marker.
+struct DictPose {
+    int32_t id_offset;
+    double len;  // the dictionary's default marker length (its own, else the call's)
+};
+
+struct DictMergeArgs {
+    int n_dicts;
+    size_t dict_stride;        // [n_dicts] of per-dictionary lists, dict_stride markers apart
+    const int32_t* count;      // [n_dicts][F]
+    const int32_t* ids;        // [n_dicts][F][max_markers]
+    const float* corners;      // [n_dicts][F][max_markers][8]
+    int F, max_markers;
+    DictPose dp[FID_MAX_DICTIONARIES];
+    int do_pose;
+    Camera cam;
+    int n_override;
+    const int32_t* override_ids;
+    const double* override_lens;
+    int32_t* out_count;        // [F]
+    int32_t* out_ids;          // [F][max_markers]
+    float* out_corners;        // [F][max_markers][8]
+    int32_t* out_dict;         // [F][max_markers]
+    fid_transform* out_tf;     // [F][max_markers]
+    struct fid_pose_hypotheses* out_hyp;  // [F][max_markers] or nullptr
+    Counters* counters;
+};
+
+#define DICT_MERGE_THREADS 64
+
+__global__ void __launch_bounds__(DICT_MERGE_THREADS) k_dict_merge(const DictMergeArgs a) {
+    __shared__ int s_off[FID_MAX_DICTIONARIES + 1];
+    const int f = blockIdx.x;
+    if (threadIdx.x == 0) {
+        int total = 0;
+        for (int d = 0; d < a.n_dicts; d++) {
+            s_off[d] = total;
+            total += a.count[(size_t)d * a.F + f];
+        }
+        const int cap = a.max_markers < FID_MAX_MARKERS ? a.max_markers : FID_MAX_MARKERS;
+        if (total > cap) {
+            atomicOr(&a.counters->overflow, 32u);
+            total = cap;
+        }
+        s_off[a.n_dicts] = total;
+        a.out_count[f] = total;
+    }
+    __syncthreads();
+    const int n = s_off[a.n_dicts];
+    for (int m = threadIdx.x; m < n; m += DICT_MERGE_THREADS) {
+        int d = 0;
+        while (m >= s_off[d + 1]) d++;
+        const size_t src = (size_t)d * a.dict_stride + (size_t)f * a.max_markers + (m - s_off[d]);
+        const size_t o = (size_t)f * a.max_markers + m;
+        const int id = a.ids[src];
+        a.out_ids[o] = id;
+        a.out_dict[o] = d;
+        float* oc = a.out_corners + o * 8;
+        for (int k = 0; k < 8; k++) oc[k] = a.corners[src * 8 + k];
+        if (!a.do_pose) continue;
+        const int pub = id + a.dp[d].id_offset;
+        const double len = marker_len_of(pub, a.dp[d].len, a.n_override, a.override_ids, a.override_lens);
+        PoseOut po;
+        solve_marker_pose(oc, a.cam, (float)len, a.dp[d].len, &po);
+        fid_transform t;
+        t.fiducial_id = pub;
+        t.reserved = po.lm_iters;
+        for (int k = 0; k < 3; k++) {
+            t.translation[k] = po.tvec[k];
+            t.rvec[k] = po.rvec[k];
+        }
+        for (int k = 0; k < 4; k++) t.rotation[k] = po.quat[k];
+        t.image_error = po.image_error;
+        t.object_error = po.object_error;
+        t.fiducial_area = po.area;
+        a.out_tf[o] = t;
+        if (a.out_hyp) {
+            PoseHypOut ho;
+            solve_marker_hypotheses(oc, a.cam, (float)len, po.rvec, &ho);
+            pack_hypotheses(pub, ho, a.out_hyp + o);
+        }
+    }
+}
+
 }  // namespace fid

@@ -79,6 +79,17 @@ class FiducialsNode {
         check(fid_default_params(&p), "fid_default_params");  // aruco_detect.cpp:690-727
         p.dictionary = dictionary;                            // :611
         check(fid_create(&p, device, max_width, max_height, 1, &det), "fid_create");
+        specs.push_back(fid_dictionary_spec{dictionary, 0, 0.0});
+    }
+
+    // Further dictionaries after `dictionary` (new, no reference counterpart; a ROS binding would read them from parameters next to
+    // `dictionary`): each with an id offset, so the published fiducial_id is id + id_offset, and a marker length (0 = fiducial_len).
+    // The messages, ignoreIds and fiducialLens then use published ids.  Detection is detectMarkersMultiDict (fid_detect_multi_dict).
+    void setDictionaries(const std::vector<fid_dictionary_spec>& extra) {
+        std::vector<fid_dictionary_spec> all(1, specs[0]);
+        all.insert(all.end(), extra.begin(), extra.end());
+        check(fid_set_dictionaries(det, (int)all.size(), all.data()), "fid_set_dictionaries");
+        specs = all;
     }
     ~FiducialsNode() {
         if (det) fid_destroy(det);
@@ -90,7 +101,8 @@ class FiducialsNode {
     // select the corner refinement method as the reference does (:274-281, same rule at start-up :700-711)
     void configCallback(fid_params p, bool doCornerRefinement, bool cornerRefinementSubpix) {
         p.cornerRefinementMethod = doCornerRefinement ? (cornerRefinementSubpix ? 1 /* SUBPIX */ : 2 /* CONTOUR */) : 0 /* NONE */;
-        check(fid_set_params(det, &p), "fid_set_params");
+        check(fid_set_params(det, &p), "fid_set_params");  // replaces the first dictionary, keeps the others
+        specs[0].dictionary = p.dictionary;
     }
 
     // camInfoCallback, aruco_detect.cpp:307-330
@@ -113,14 +125,19 @@ class FiducialsNode {
         fva->fiducials.clear();
         ids.assign(FID_MAX_MARKERS, 0);
         corners.assign(FID_MAX_MARKERS * 8, 0.f);
+        dictIdx.assign(FID_MAX_MARKERS, 0);
         int n = 0;
-        if (fid_detect(det, bgr, width, height, stride, FID_MAX_MARKERS, &n, ids.data(), corners.data()) != FID_OK) return false;  // frame dropped (:389-394)
+        const int rc = specs.size() > 1 ? fid_detect_multi_dict(det, bgr, width, height, stride, FID_MAX_MARKERS, &n, ids.data(), corners.data(), dictIdx.data())
+                                        : fid_detect(det, bgr, width, height, stride, FID_MAX_MARKERS, &n, ids.data(), corners.data());
+        if (rc != FID_OK) return false;  // frame dropped (:389-394)
         ids.resize(n);
         corners.resize((size_t)n * 8);
+        dictIdx.resize(n);
         for (int i = 0; i < n; i++) {
-            if (std::count(ignoreIds.begin(), ignoreIds.end(), ids[i]) != 0) continue;  // :359-364
+            const int pub = ids[i] + specs[dictIdx[i]].id_offset;
+            if (std::count(ignoreIds.begin(), ignoreIds.end(), pub) != 0) continue;  // :359-364
             Fiducial f;
-            f.fiducial_id = ids[i];
+            f.fiducial_id = pub;
             const float* c = &corners[(size_t)i * 8];
             f.x0 = c[0]; f.y0 = c[1]; f.x1 = c[2]; f.y1 = c[3]; f.x2 = c[4]; f.y2 = c[5]; f.x3 = c[6]; f.y3 = c[7];  // :366-376
             fva->fiducials.push_back(f);
@@ -144,8 +161,23 @@ class FiducialsNode {
             oi.push_back(kv.first);
             ol.push_back(kv.second);
         }
+        // one fid_pose per dictionary, on its markers' published ids and its length (one call over all markers with one dictionary)
         std::vector<fid_transform> out(ids.size());
-        if (fid_pose(det, (int)ids.size(), ids.data(), corners.data(), &cam, fiducial_len, (int)oi.size(), oi.data(), ol.data(), out.data()) != FID_OK) return true;
+        for (size_t d = 0; d < specs.size(); d++) {
+            std::vector<int32_t> gi, pos;
+            std::vector<float> gc;
+            for (size_t i = 0; i < ids.size(); i++) {
+                if (dictIdx[i] != (int)d) continue;
+                pos.push_back((int32_t)i);
+                gi.push_back(ids[i] + specs[d].id_offset);
+                gc.insert(gc.end(), corners.begin() + i * 8, corners.begin() + i * 8 + 8);
+            }
+            if (gi.empty()) continue;
+            std::vector<fid_transform> g(gi.size());
+            const double len = specs[d].fiducial_len > 0 ? specs[d].fiducial_len : fiducial_len;
+            if (fid_pose(det, (int)gi.size(), gi.data(), gc.data(), &cam, len, (int)oi.size(), oi.data(), ol.data(), g.data()) != FID_OK) return true;
+            for (size_t k = 0; k < pos.size(); k++) out[pos[k]] = g[k];
+        }
         for (const fid_transform& t : out) {
             if (std::count(ignoreIds.begin(), ignoreIds.end(), t.fiducial_id) != 0) continue;  // :440
             FiducialTransform ft;
@@ -185,6 +217,8 @@ class FiducialsNode {
     fid_camera cam{};
     std::vector<int32_t> ids;
     std::vector<float> corners;
+    std::vector<int32_t> dictIdx;            // each marker's dictionary (all 0 with one dictionary)
+    std::vector<fid_dictionary_spec> specs;  // entry 0 = the constructor's dictionary
     Header last;
 };
 

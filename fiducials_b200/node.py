@@ -155,6 +155,36 @@ class Detector:
                                               C.cast(tfs, C.c_void_p) if tfs is not None else None), "fid_collect_batch")
         return counts, ids, corners, tfs
 
+    def set_dictionaries(self, specs):
+        """fid_set_dictionaries: specs = [(dictionary, id_offset, fiducial_len), ...] (a bare int is (dictionary, 0, 0.0)); entry 0's
+        dictionary becomes params.dictionary.  Batches then detect with every dictionary (detectMarkersMultiDict)."""
+        specs = [(s, 0, 0.0) if isinstance(s, (int, np.integer)) else tuple(s) for s in specs]
+        arr = (_lib.fid_dictionary_spec * max(len(specs), 1))()
+        for i, (d, off, ln) in enumerate(specs):
+            arr[i] = _lib.fid_dictionary_spec(int(d), int(off), float(ln))
+        _lib.check(self.lib.fid_set_dictionaries(self.h, len(specs), C.cast(arr, C.c_void_p)), "fid_set_dictionaries")
+        self.params.dictionary = int(specs[0][0])
+
+    def detect_multi_dict(self, bgr: np.ndarray):
+        """fid_detect_multi_dict: (ids int32[n], corners float32[n,4,2], dict_indices int32[n])."""
+        bgr = np.ascontiguousarray(bgr, np.uint8)
+        H, W = bgr.shape[:2]
+        ids = np.zeros(MAXM, np.int32)
+        corners = np.zeros((MAXM, 8), np.float32)
+        di = np.zeros(MAXM, np.int32)
+        n = C.c_int(0)
+        _lib.check(self.lib.fid_detect_multi_dict(self.h, bgr.ctypes.data_as(C.c_void_p), W, H, W * self.bpp, MAXM, C.byref(n), ids.ctypes.data_as(C.c_void_p),
+                                                  corners.ctypes.data_as(C.c_void_p), di.ctypes.data_as(C.c_void_p)), "fid_detect_multi_dict")
+        return ids[: n.value].copy(), corners[: n.value].reshape(-1, 4, 2).copy(), di[: n.value].copy()
+
+    def last_dict_indices(self, max_markers=MAXM):
+        """fid_last_dict_indices: int32 [n_frames, max_markers], laid out like the batch's ids."""
+        nf = C.c_int(0)
+        _lib.check(self.lib.fid_last_dict_indices(self.h, max_markers, C.byref(nf), None), "fid_last_dict_indices")
+        out = np.zeros((nf.value, max_markers), np.int32)
+        _lib.check(self.lib.fid_last_dict_indices(self.h, max_markers, C.byref(nf), out.ctypes.data_as(C.c_void_p)), "fid_last_dict_indices")
+        return out
+
     def set_pose_hypotheses(self, enable: bool):
         """fid_set_pose_hypotheses: batches submitted from now on also compute both planar pose solutions of every marker."""
         _lib.check(self.lib.fid_set_pose_hypotheses(self.h, int(bool(enable))), "fid_set_pose_hypotheses")
@@ -426,7 +456,7 @@ class FiducialsNode:
 
     def __init__(self, dictionary=7, fiducial_len=0.14, ignore_fiducials: Iterable[int] = (), fiducial_len_override: Optional[Dict[int, float]] = None,
                  do_pose_estimation=True, device=0, max_width=1920, max_height=1080, max_batch=1, doCornerRefinement=True, cornerRefinementSubPix=True, pose_hypotheses=False,
-                 boards=(), charuco_boards=(), refine_markers=None, diamonds=None, **detector_params):
+                 boards=(), charuco_boards=(), refine_markers=None, diamonds=None, dictionaries=(), **detector_params):
         # doCornerRefinement / cornerRefinementSubPix -> cornerRefinementMethod NONE / SUBPIX / CONTOUR (:700-711, configCallback :274-281)
         if refine_markers is not None and not boards and not charuco_boards:
             raise ValueError("refine_markers needs boards or charuco_boards")
@@ -436,6 +466,13 @@ class FiducialsNode:
         self.ignoreIds = set(int(i) for i in ignore_fiducials)  # :540-571
         self.fiducialLens = dict(fiducial_len_override or {})  # :627-660
         self.det = Detector(default_params(dictionary=dictionary, **detector_params), device, max_width, max_height, max_batch)
+        # further dictionaries (new, no reference counterpart): dictionaries = [(dictionary, id_offset, fiducial_len), ...] after
+        # `dictionary`; detection is detectMarkersMultiDict, the messages carry published ids (id + id_offset), and ignore_fiducials /
+        # fiducial_len_override are keyed by them; a dictionary's fiducial_len of 0 means fiducial_len
+        self.dictSpecs = [(int(dictionary), 0, 0.0)] + [(int(d), int(o), float(l)) for d, o, l in dictionaries]
+        if len(self.dictSpecs) > 1:
+            self.det.set_dictionaries(self.dictSpecs)
+        self.dictIdx = np.zeros(0, np.int32)
         # both planar pose solutions of every marker (new, no reference counterpart): when on, the pose results carry an extra
         # attribute `pose_hypotheses` = {fiducial_id: fid_pose_hypotheses record}; their message fields are unchanged
         self.poseHypotheses = bool(pose_hypotheses)
@@ -502,13 +539,17 @@ class FiducialsNode:
                 self.ids, self.corners = ids[0, :n].copy(), corners[0, :n].copy()
                 idx, brd, _, _ = self.det.last_marker_refinement()[0]
                 self._recovered = self._recovered_of(self.ids, idx, brd)
+            elif len(self.dictSpecs) > 1:
+                self.ids, self.corners, self.dictIdx = self.det.detect_multi_dict(bgr)
             else:
                 self.ids, self.corners = self.det.detect(bgr)  # :350
         except _lib.FidError:
             return None  # frame dropped (:389-394)
+        if len(self.dictSpecs) == 1:
+            self.dictIdx = np.zeros(len(self.ids), np.int32)
         if self.charucoBoards or self.diamondGeometry is not None:
             self._last_frame = np.ascontiguousarray(bgr, np.uint8)
-        for i, fid in enumerate(self.ids.tolist()):
+        for i, fid in enumerate(self._published().tolist()):
             if fid in self.ignoreIds:
                 continue  # :359-364
             c = self.corners[i]
@@ -517,6 +558,24 @@ class FiducialsNode:
             fva.recovered = self._recovered
         self._last_header = header
         return fva
+
+    def _published(self):
+        """The published ids of the last imageCallback's markers: id + their dictionary's id_offset."""
+        offsets = np.array([s[1] for s in self.dictSpecs], np.int32)
+        return self.ids + offsets[self.dictIdx]
+
+    def _per_dictionary(self, solve):
+        """solve(published ids, corners, length) once per dictionary over its markers; the records in marker order."""
+        if len(self.dictSpecs) == 1:
+            return solve(self.ids, self.corners, self.fiducial_len)
+        out = [None] * len(self.ids)
+        pub = self._published()
+        for d, (_, _, ln) in enumerate(self.dictSpecs):
+            sel = np.where(self.dictIdx == d)[0]
+            if len(sel):
+                for m, r in zip(sel.tolist(), solve(pub[sel], self.corners[sel], ln if ln > 0 else self.fiducial_len)):
+                    out[m] = r
+        return out
 
     def _recovered_of(self, ids, idx, boards):
         """The frame's recovered markers (its last len(idx) markers) as (fiducial_id, board), without the ignored ids."""
@@ -533,8 +592,8 @@ class FiducialsNode:
         if not self.haveCamInfo:
             return None  # :417-422
         try:
-            tfs = self.det.pose(self.ids, self.corners, self.K, self.D, self.fiducial_len, self.fiducialLens)
-            hyps = self.det.pose_hypotheses(self.ids, self.corners, self.K, self.D, self.fiducial_len, self.fiducialLens) if self.poseHypotheses else None
+            tfs = self._per_dictionary(lambda i, c, ln: self.det.pose(i, c, self.K, self.D, ln, self.fiducialLens))
+            hyps = self._per_dictionary(lambda i, c, ln: self.det.pose_hypotheses(i, c, self.K, self.D, ln, self.fiducialLens)) if self.poseHypotheses else None
             boards = self.det.board_poses(self.ids, self.corners, self.K, self.D) if self.boards else None
             charuco = self.det.charuco(self._last_frame, self.ids, self.corners, self.K, self.D) if self.charucoBoards and self._last_frame is not None else None
             diamonds = self.det.diamonds(self._last_frame, self.ids, self.corners, self.K, self.D) if self.diamondGeometry is not None and self._last_frame is not None else None

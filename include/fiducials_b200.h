@@ -340,6 +340,39 @@ int fid_detect_diamonds(fid_detector* h, const uint8_t* bgr, int width, int heig
  * that batch ran without diamonds; FID_ERR_CAPACITY, with nothing written, if a frame has more than max_diamonds. */
 int fid_last_diamonds(fid_detector* h, int max_diamonds, int* n_frames, int32_t* counts, fid_diamond* out);
 
+/* Several dictionaries in one pass: cv::aruco::ArucoDetector(dictionaries) and detectMarkersMultiDict (OpenCV >= 4.12).  The
+ * threshold, border walk and quad stages run once per frame; grouping runs once per run of equal marker sizes, and identification,
+ * the candidate hierarchy, corner refinement and the pose once per dictionary.  The markers are the concatenation, in list order,
+ * of what detectMarkers returns for each dictionary alone (a dictionary listed twice reports its markers twice).
+ *   dictionary    the OpenCV enum (the fid_params.dictionary values)
+ *   id_offset     fid_transform.fiducial_id = id + id_offset ("published id"), so that two families with equal raw ids stay apart
+ *                 in the map; ids and corners stay cv2's raw values
+ *   fiducial_len  metres, 0 = the call's fiducial_len.  A marker's length is the fiducial_len_override entry of its published id,
+ *                 else this length if > 0, else the call's; object_error uses this length (else the call's) as the default length. */
+#define FID_MAX_DICTIONARIES 8
+typedef struct fid_dictionary_spec {
+    int32_t dictionary;
+    int32_t id_offset;
+    double fiducial_len;
+} fid_dictionary_spec;
+/* Replace the handle's dictionary list (1..FID_MAX_DICTIONARIES entries); entry 0's dictionary becomes fid_params.dictionary, and
+ * fid_set_params later replaces entry 0's dictionary and keeps the others (cv2's setDictionary).  Every entry must pass the limits
+ * fid_create applies to fid_params.dictionary: FID_ERR_UNSUPPORTED / FID_ERR_INVALID_ARG otherwise, also for a length that is
+ * negative or not finite or an offset with which id + id_offset overflows int32, each with the handle unchanged.  A handle is in
+ * multi-dictionary mode when the list has more than one entry or entry 0 has an offset or a length; the batch calls then detect
+ * with every dictionary.  Marker boards, ChArUco boards, batch marker refinement and diamonds are refused (FID_ERR_UNSUPPORTED,
+ * nothing changed) in that mode, in both directions.  Not while batches are in flight. */
+int fid_set_dictionaries(fid_detector* h, int n, const fid_dictionary_spec* specs);
+/* detectMarkersMultiDict for one frame (fid_detect's arguments): ids, corners and dict_indices (may be NULL) [n], max_markers a
+ * total over all dictionaries (FID_ERR_CAPACITY with the first max_markers written beyond it).  fid_detect stays detectMarkers
+ * with dictionary 0 alone, as cv2's detectMarkers on a detector with several dictionaries. */
+int fid_detect_multi_dict(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int max_markers, int* n, int32_t* ids, float* corners,
+                          int32_t* dict_indices);
+/* The dictionary index of every marker of the batch most recently returned by fid_collect_batch / fid_detect_pose_batch, dense
+ * [n_frames][max_markers] (all zeros without multi-dictionary mode).  *n_frames = that batch's frame count; out may be NULL to query
+ * it.  FID_ERR_INVALID_ARG before the first batch; FID_ERR_CAPACITY, with nothing written, if a frame has more than max_markers. */
+int fid_last_dict_indices(fid_detector* h, int max_markers, int* n_frames, int32_t* out);
+
 /* Pixel format of the frames handed to every entry point that takes `bgr` (default FID_ENC_BGR8).  The
  * reference converts whatever the camera publishes with cv_bridge::toCvCopy(msg, BGR8)
  * (aruco_detect.cpp:348) before detectMarkers turns it into gray again; the library takes the camera's own
@@ -392,7 +425,8 @@ int fid_debug_rejected(fid_detector* h, int max_rejected, int* n, float* rejecte
 /* Per-stage device times (milliseconds, CUDA events) of the last batch call:
  * [0] h2d copy, [1] threshold (+ start cracks), [2] unused (reads 0), [3] border walk, [4] chain emit, [5] polygon+filters,
  * [6] group, [7] identify, [8] subpix+pose, [9] unused, [10] d2h, [11..18] the border-walk rounds
- * (unused rounds read 0); n_stages returns 19. */
+ * (unused rounds read 0); n_stages returns 19.  In multi-dictionary mode (fid_set_dictionaries) the per-dictionary launches interleave:
+ * [6] then holds grouping, identification and the output stage of every dictionary, [7] reads 0 and [8] is the merge (k_dict_merge). */
 int fid_last_stage_ms(fid_detector* h, float* ms, int max_stages, int* n_stages);
 /* Work counters of the last batch call: [0] start cracks, [1] walk survivors (contours in range),
  * [2] contour points emitted, [3] quad candidates, [4] candidates selected, [5] markers,
