@@ -16,6 +16,7 @@
 #include "start_prune_table.h"
 #include "kernels_threshold_mma.cuh"
 #include "kernels_marker.cuh"
+#include "kernels_aruco3.cuh"
 #include "params_host.h"
 
 using namespace fid;
@@ -75,6 +76,10 @@ struct Slot {
     int32_t* d_md_ids = nullptr;                       // [n_dicts][max_batch][max_markers]
     float* d_md_corners = nullptr;                     // [n_dicts][max_batch][max_markers][8]
     int32_t* d_out_dict = nullptr;                     // [max_batch][max_markers]          k_dict_merge
+    // fid_set_aruco3: allocated by the first enable (level 0 of the pyramid is d_gray)
+    uint8_t* d_a3_pyr = nullptr;                       // [max_batch][levels 1.. of the largest frame]
+    uint8_t* d_a3_seg = nullptr;                       // [max_batch][the largest segmentation plane of the mode's parameters]
+    size_t a3_pyr_cap = 0, a3_seg_cap = 0;             // their sizes in bytes; fid_set_aruco3 grows them
     // pinned host mirrors
     int32_t* h_out_count = nullptr;
     int32_t* h_out_ids = nullptr;
@@ -209,6 +214,7 @@ struct fid_detector {
     bool last_di_valid = false;                      // fid_last_dict_indices
     int last_di_frames = 0, last_di_stride = 0;
     std::vector<int32_t> last_di_counts, last_di;    // [last_di_frames][last_di_stride]
+    fid_aruco3_params aruco3{};                      // useAruco3Detection (fid_set_aruco3); enable = 0: off
     bool detected_multi = false;                     // slot 0 holds fid_detect_multi_dict's candidates, not detectMarkers'
     int32_t* d_dbg_rej_n = nullptr;                  // fid_debug_rejected: count, then [max_sel][8] floats
     float* d_dbg_rej = nullptr;
@@ -323,8 +329,10 @@ static int configure_kernels(fid_detector* h) {
     CK(cudaFuncSetAttribute(k_threshold_mma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TM_SMEM_BYTES));
     CK(cudaFuncSetAttribute(k_threshold_mma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TM_SMEM_BYTES));
     CK(cudaFuncSetAttribute(k_sort_group, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)group_smem(FID_GROUP_MAX_RAW)));
-    CK(cudaFuncSetAttribute(k_identify_retry, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kMaxDictMarkers * 4 * 8 + IDENT_WARPS * 256 * 4 + IDENT_WARPS * FID_MAX_WARP_SIDE_SQ)));
-    CK(cudaFuncSetAttribute(k_identify_first, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kMaxDictMarkers * 4 * 8 + IDENT0_WARPS * 256 * 4 + IDENT0_WARPS * FID_MAX_WARP_SIDE_SQ)));
+    for (auto k : {k_identify_retry<false>, k_identify_retry<true>})
+        CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kMaxDictMarkers * 4 * 8 + IDENT_WARPS * 256 * 4 + IDENT_WARPS * FID_MAX_WARP_SIDE_SQ)));
+    for (auto k : {k_identify_first<false>, k_identify_first<true>})
+        CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kMaxDictMarkers * 4 * 8 + IDENT0_WARPS * 256 * 4 + IDENT0_WARPS * FID_MAX_WARP_SIDE_SQ)));
     return FID_OK;
 }
 
@@ -399,7 +407,7 @@ static void free_slot(Slot& s) {
                      s.fs.sel_idx,    s.d_nsel,          s.d_nrawc,         s.d_cand_id,      s.d_cand_corners, s.d_out_count,    s.d_out_ids,     s.d_out_corners,
                      s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp, s.d_out_board, s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy,
                      s.d_rej_n,       s.d_rej,           s.d_mr_nrec,       s.d_mr_idx,       s.d_mr_board,    s.d_dia_n,       s.d_dia,
-                     s.d_md_count,    s.d_md_ids,        s.d_md_corners,    s.d_out_dict};
+                     s.d_md_count,    s.d_md_ids,        s.d_md_corners,    s.d_out_dict,     s.d_a3_pyr,      s.d_a3_seg};
     for (void* p : dptrs)
         if (p) cudaFree(p);
     void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp, s.h_out_board, s.h_out_ch, s.h_out_ch_ids, s.h_out_ch_xy,
@@ -627,7 +635,7 @@ extern "C" int fid_set_dictionaries(fid_detector* h, int n, const fid_dictionary
         if ((int64_t)specs[d].id_offset + dp[d].n_markers - 1 > INT32_MAX) return FID_ERR_INVALID_ARG;  // a published id would overflow
     }
     const bool multi = n > 1 || specs[0].id_offset != 0 || specs[0].fiducial_len > 0;
-    if (multi && (h->n_boards || h->n_charuco || h->batch_refine || h->diamond.enable)) return FID_ERR_UNSUPPORTED;
+    if (multi && (h->n_boards || h->n_charuco || h->batch_refine || h->diamond.enable || h->aruco3.enable)) return FID_ERR_UNSUPPORTED;
     CK(cudaSetDevice(h->device));
     if (multi) {  // (a failed allocation leaves the handle as it was; the next call completes it)
         const size_t F = h->max_batch, M = F * h->max_markers, ND = FID_MAX_DICTIONARIES;
@@ -808,11 +816,64 @@ static DiamondArgs diamond_args(const fid_detector* h, const uint8_t* src, size_
 // A batch refines only with the batch switch, the refinement parameters and a board to refine against.
 static bool batch_refines(const fid_detector* h) { return h->batch_refine && h->mrefine.enable && h->n_boards + h->n_charuco > 0; }
 
+// useAruco3Detection (fid_set_aruco3): the gray plane (k_gray into d_gray, level 0), the pyrDown levels and the segmentation plane
+// of nf frames.  Returns the number of launches.
+static int enqueue_aruco3_planes(const fid_detector* h, Slot& s, cudaStream_t st, int nf, const FrameGeom& g, const uint8_t* d_bgr, const A3Geom& ag) {
+    GrayArgs ga{};
+    ga.bgr = d_bgr;
+    ga.gray = s.d_gray;
+    ga.W = g.W;
+    ga.H = g.H;
+    ga.n_frames = nf;
+    ga.bgr_row_stride = g.bgr_row_stride;
+    ga.bgr_frame_stride = g.bgr_frame_stride;
+    ga.gray_pitch = g.gray_pitch;
+    ga.gray_frame_stride = g.gray_frame_stride;
+    ga.enc = h->enc;
+    const long long gq = (long long)nf * g.H * ((g.W + 3) / 4);
+    k_gray<<<(unsigned int)((gq + 255) / 256), 256, 0, st>>>(ga);
+    int launches = 1;
+    for (int l = 1; l < ag.n_levels; l++) {
+        A3PlaneArgs a{};
+        a.src = l == 1 ? s.d_gray : s.d_a3_pyr + ag.lv[l - 1].off;
+        a.src_pitch = ag.lv[l - 1].pitch;
+        a.src_frame_stride = l == 1 ? g.gray_frame_stride : ag.pyr_frame_bytes;
+        a.sw = ag.lv[l - 1].W;
+        a.sh = ag.lv[l - 1].H;
+        a.dst = s.d_a3_pyr + ag.lv[l].off;
+        a.dst_pitch = ag.lv[l].pitch;
+        a.dst_frame_stride = ag.pyr_frame_bytes;
+        a.dw = ag.lv[l].W;
+        a.dh = ag.lv[l].H;
+        a.n_frames = nf;
+        k_a3_pyr_down<<<dim3((a.dw + 255) / 256, a.dh, nf), 256, 0, st>>>(a);
+        launches++;
+    }
+    if (ag.resized) {
+        A3PlaneArgs a{};
+        a.src = s.d_gray;
+        a.src_pitch = g.gray_pitch;
+        a.src_frame_stride = g.gray_frame_stride;
+        a.sw = g.W;
+        a.sh = g.H;
+        a.dst = s.d_a3_seg;
+        a.dst_pitch = ag.seg_w;
+        a.dst_frame_stride = (size_t)ag.seg_w * ag.seg_h;
+        a.dw = ag.seg_w;
+        a.dh = ag.seg_h;
+        a.n_frames = nf;
+        a.scale_x = 1.0 / ((double)ag.seg_w / g.W);
+        a.scale_y = 1.0 / ((double)ag.seg_h / g.H);
+        k_a3_resize<<<dim3((a.dw + 255) / 256, a.dh, nf), 256, 0, st>>>(a);
+        launches++;
+    }
+    return launches;
+}
+
 static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, const FrameGeom& g, const uint8_t* d_bgr, const fid_camera* cam, double fiducial_len,
                             int n_override, int stop_after /* -1 = all */, const Slot* prev = nullptr, bool refine = false, bool diamonds = false,
                             bool multi = false) {
     const DevParams& P = h->P;
-    const int W = g.W, H = g.H;
     int launches = 0;
     CK(cudaMemsetAsync(s.d_counters, 0, sizeof(Counters), st));
     CK(cudaMemsetAsync(s.d_nraw, 0, sizeof(unsigned int) * nf, st));
@@ -821,35 +882,52 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
     // throughput-bound stages of the other instead of under its own twin
     if (prev && (h->stagger & 1)) CK(cudaStreamWaitEvent(st, prev->ev[ST_MASKS], 0));
     CK(cudaEventRecord(s.ev[ST_THRESH], st));
+    // useAruco3Detection: the stages up to k_finish run on the segmentation plane, a mono8 frame of its own size (gs, seg_src).
+    // The threshold-only runs (fid_debug_threshold, fid_debug_time_threshold) stay on the full frame.
+    const bool a3 = h->aruco3.enable != 0 && stop_after != ST_THRESH;
+    A3Geom ag{};
+    FrameGeom gs = g;
+    const uint8_t* seg_src = d_bgr;
+    int seg_enc = h->enc;
+    if (a3) {
+        if (!a3_geometry(g.W, g.H, h->aruco3.minSideLengthCanonicalImg, h->aruco3.minMarkerLengthRatioOriginalImg, &ag)) return FID_ERR_INVALID_ARG;
+        if ((size_t)nf * ag.pyr_frame_bytes > s.a3_pyr_cap || (ag.resized && (size_t)nf * ag.seg_w * ag.seg_h > s.a3_seg_cap)) return FID_ERR_CAPACITY;  // see a3_plane_bytes
+        launches += enqueue_aruco3_planes(h, s, st, nf, g, d_bgr, ag);
+        seg_src = ag.resized ? s.d_a3_seg : s.d_gray;
+        const size_t pitch = ag.resized ? (size_t)ag.seg_w : (size_t)g.gray_pitch;
+        gs = make_geom(h, ag.seg_w, ag.seg_h, pitch, pitch * ag.seg_h);
+        seg_enc = FID_ENC_MONO8;
+    }
+    const int W = gs.W, H = gs.H;
     {  // threshold stage: gray + 13 adaptive thresholds -> halo tiles + start cracks
         bool fast = P.n_scales == 13;
         for (int i = 0; i < P.n_scales; i++) fast = fast && P.win[i] == 3 + 4 * i;
         if (fast && h->thresh_mode == 1) {
             // tensor-core kernel: persistent, one CTA per SM; BGR staged by TMA where the layout allows
             ThreshMmaArgs a{};
-            a.src = d_bgr;
-            a.enc = h->enc;
-            a.bpp = h->bpp;
-            a.row_stride = g.bgr_row_stride;
-            a.frame_stride = g.bgr_frame_stride;
+            a.src = seg_src;
+            a.enc = seg_enc;
+            a.bpp = seg_enc == FID_ENC_MONO8 ? 1 : 3;
+            a.row_stride = gs.bgr_row_stride;
+            a.frame_stride = gs.bgr_frame_stride;
             a.halo = s.d_halo;
             a.W = W;
             a.H = H;
             a.n_frames = nf;
-            a.halo_tpr = g.halo_tpr;
-            a.halo_tiles_y = g.halo_tiles_y;
-            a.halo_scale_stride = g.halo_scale_stride;
-            a.halo_frame_stride = g.halo_frame_stride;
+            a.halo_tpr = gs.halo_tpr;
+            a.halo_tiles_y = gs.halo_tiles_y;
+            a.halo_scale_stride = gs.halo_scale_stride;
+            a.halo_frame_stride = gs.halo_frame_stride;
             a.thresh_c = P.thresh_c;
-            a.tiles_x = (g.halo_tpr + THR_TILES_X - 1) / THR_TILES_X;
-            a.tiles_y = (g.halo_tiles_y + THR_TILES_Y - 1) / THR_TILES_Y;
+            a.tiles_x = (gs.halo_tpr + THR_TILES_X - 1) / THR_TILES_X;
+            a.tiles_y = (gs.halo_tiles_y + THR_TILES_Y - 1) / THR_TILES_Y;
             a.starts = s.d_starts;
             a.counters = s.d_counters;
             a.max_starts = h->max_starts;
             CUtensorMap tmap;
             memset(&tmap, 0, sizeof(tmap));
             static const bool tma_off = getenv("FID_THRESH_TMA") && atoi(getenv("FID_THRESH_TMA")) == 0;  // debugging switch
-            a.use_tma = (!tma_off && h->enc != FID_ENC_MONO8 && make_bgr_tensor_map(&tmap, d_bgr, W, H, nf, g.bgr_row_stride, g.bgr_frame_stride)) ? 1 : 0;
+            a.use_tma = (!tma_off && seg_enc != FID_ENC_MONO8 && make_bgr_tensor_map(&tmap, seg_src, W, H, nf, gs.bgr_row_stride, gs.bgr_frame_stride)) ? 1 : 0;
             const long long total = (long long)a.tiles_x * a.tiles_y * nf;
             const int grid = (int)std::min<long long>(total, h->sm_count);
             static const bool prof_on = getenv("FID_THRESH_PROF") && atoi(getenv("FID_THRESH_PROF")) != 0;  // debugging: per-warp wait cycles
@@ -877,19 +955,19 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
             }
         } else {
             ThreshArgs a{};
-            a.src = d_bgr;
-            a.src_row_stride = g.bgr_row_stride;
-            a.src_frame_stride = g.bgr_frame_stride;
-            a.enc = h->enc;
-            a.aligned4 = (W % 4 == 0) && (g.bgr_row_stride % 4 == 0) && (g.bgr_frame_stride % 4 == 0) && ((uintptr_t)d_bgr % 4 == 0);
+            a.src = seg_src;
+            a.src_row_stride = gs.bgr_row_stride;
+            a.src_frame_stride = gs.bgr_frame_stride;
+            a.enc = seg_enc;
+            a.aligned4 = (W % 4 == 0) && (gs.bgr_row_stride % 4 == 0) && (gs.bgr_frame_stride % 4 == 0) && ((uintptr_t)seg_src % 4 == 0);
             a.halo = s.d_halo;
             a.W = W;
             a.H = H;
             a.n_frames = nf;
-            a.halo_tpr = g.halo_tpr;
-            a.halo_tiles_y = g.halo_tiles_y;
-            a.halo_scale_stride = g.halo_scale_stride;
-            a.halo_frame_stride = g.halo_frame_stride;
+            a.halo_tpr = gs.halo_tpr;
+            a.halo_tiles_y = gs.halo_tiles_y;
+            a.halo_scale_stride = gs.halo_scale_stride;
+            a.halo_frame_stride = gs.halo_frame_stride;
             a.n_scales = P.n_scales;
             a.r_max = r_max_of(P);
             a.thresh_c = P.thresh_c;
@@ -898,7 +976,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
             a.max_starts = h->max_starts;
             a.prune = h->start_prune ? h->d_prune : nullptr;
             for (int i = 0; i < P.n_scales; i++) a.win[i] = P.win[i];
-            dim3 grid((g.halo_tpr + THR_TILES_X - 1) / THR_TILES_X, (g.halo_tiles_y + THR_TILES_Y - 1) / THR_TILES_Y, nf);
+            dim3 grid((gs.halo_tpr + THR_TILES_X - 1) / THR_TILES_X, (gs.halo_tiles_y + THR_TILES_Y - 1) / THR_TILES_Y, nf);
             if (a.prune) {
                 if (fast)
                     launch_prio(k_threshold<true, true>, grid, dim3(THR_THREADS), thresh_smem_bytes(THR_FAST_R), st, 0, a);
@@ -917,7 +995,8 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
     CK(cudaEventRecord(s.ev[ST_WALK], st));
     if (prev && (h->stagger & 2)) CK(cudaStreamWaitEvent(st, prev->ev[ST_EMIT], 0));
     const int mx = W > H ? W : H;
-    const int min_len = (int)(P.min_perimeter_rate * mx), max_len = (int)(P.max_perimeter_rate * mx);
+    // useAruco3Detection replaces minMarkerPerimeterRate by a minimum contour length of 4 * minSideLengthCanonicalImg
+    const int min_len = a3 ? 4 * h->aruco3.minSideLengthCanonicalImg : (int)(P.min_perimeter_rate * mx), max_len = (int)(P.max_perimeter_rate * mx);
     {  // walk, in rounds of growing budget
         WalkArgs a{};
         a.halo = s.d_halo;
@@ -932,7 +1011,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.max_chains = h->max_chains;
         a.max_points = h->max_points;
         a.max_queue = h->max_queue;
-        a.g = g;
+        a.g = gs;
         a.min_len = min_len;
         a.max_len = max_len;
         for (int r = 0; r < N_WALK_ROUNDS; r++) {
@@ -964,7 +1043,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.counters = s.d_counters;
         a.work_counter = &s.d_counters->emit_work;
         a.max_segs = h->max_segs;
-        a.g = g;
+        a.g = gs;
         launch_prio(k_emit, dim3(h->sm_count * h->emit_blocks_per_sm), dim3(64), 0, st, 3, a);
         launches++;
     }
@@ -1021,8 +1100,8 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.row_stride = g.bgr_row_stride;
         a.frame_stride = g.bgr_frame_stride;
         a.enc = h->enc;
-        a.W = W;
-        a.H = H;
+        a.W = g.W;
+        a.H = g.H;
         a.fs = s.fs;
         a.n_sel = s.d_nsel;
         a.max_raw = h->max_raw;
@@ -1036,8 +1115,14 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.retry_list = s.d_retry_list;
         a.counters = s.d_counters;
         // fixed grids over work lists: a grid of one block per (frame, candidate slot) is 32 768 blocks of which 1 500 have work
-        launch_prio(k_identify_first, dim3(h->sm_count * 4), dim3(IDENT0_WARPS * 32), ident_smem(Pd, IDENT0_WARPS), st, 4, a);
-        launch_prio(k_identify_retry, dim3(h->sm_count * 2), dim3(IDENT_WARPS * 32), ident_smem(Pd, IDENT_WARPS), st, 4, a);
+        if (a3) {
+            a.pyr = A3Pyramid{s.d_gray, g.gray_frame_stride, s.d_a3_pyr, s.d_raw, ag};
+            launch_prio(k_identify_first<true>, dim3(h->sm_count * 4), dim3(IDENT0_WARPS * 32), ident_smem(Pd, IDENT0_WARPS), st, 4, a);
+            launch_prio(k_identify_retry<true>, dim3(h->sm_count * 2), dim3(IDENT_WARPS * 32), ident_smem(Pd, IDENT_WARPS), st, 4, a);
+        } else {
+            launch_prio(k_identify_first<false>, dim3(h->sm_count * 4), dim3(IDENT0_WARPS * 32), ident_smem(Pd, IDENT0_WARPS), st, 4, a);
+            launch_prio(k_identify_retry<false>, dim3(h->sm_count * 2), dim3(IDENT_WARPS * 32), ident_smem(Pd, IDENT_WARPS), st, 4, a);
+        }
         launches += 2;
     };
     auto contour_refine = [&]() {  // CORNER_REFINE_CONTOUR: rewrite the decoded candidates' corners before the output stage
@@ -1059,8 +1144,8 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.row_stride = g.bgr_row_stride;
         a.frame_stride = g.bgr_frame_stride;
         a.enc = h->enc;
-        a.W = W;
-        a.H = H;
+        a.W = g.W;
+        a.H = g.H;
         a.n_sel = s.d_nsel;
         a.cand_id = s.d_cand_id;
         a.cand_corners = s.d_cand_corners;
@@ -1137,8 +1222,40 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
     CK(cudaEventRecord(s.ev[ST_IDENT], st));
     identify(P, h->d_dict);
     CK(cudaEventRecord(s.ev[ST_SUBPIX_POSE], st));
-    if (P.corner_refine == 2) contour_refine();
-    finish(P, cam, s.d_out_count, s.d_out_ids, s.d_out_corners);
+    if (a3) {  // k_finish without refinement or pose, then findCornerInPyrImage and the poses on the full-resolution corners
+        DevParams Pf = P;
+        Pf.corner_refine = 0;
+        finish(Pf, nullptr, s.d_out_count, s.d_out_ids, s.d_out_corners);
+        A3CornerArgs ca{};
+        ca.pyr = A3Pyramid{s.d_gray, g.gray_frame_stride, s.d_a3_pyr, s.d_raw, ag};
+        ca.count = s.d_out_count;
+        ca.corners = s.d_out_corners;
+        ca.max_markers = h->max_markers;
+        ca.subpix_masks = h->d_subpix_masks;
+        ca.max_iters = P.refine_max_iter;
+        ca.eps_sq = P.refine_min_acc * P.refine_min_acc;
+        launch_prio(k_a3_corners, dim3(nf), dim3(FINISH_THREADS), 0, st, 5, ca);
+        launches++;
+        if (cam) {
+            RecoveredPoseArgs pa{};
+            pa.count = s.d_out_count;
+            pa.n_rec = s.d_out_count;  // every marker of the frame
+            pa.ids = s.d_out_ids;
+            pa.corners = s.d_out_corners;
+            pa.max_markers = h->max_markers;
+            pa.cam = make_camera(cam);
+            pa.fiducial_len = fiducial_len;
+            pa.n_override = n_override;
+            pa.override_ids = h->d_override_ids;
+            pa.override_lens = h->d_override_lens;
+            pa.out_tf = s.d_out_tf;
+            launch_prio(k_recovered_pose, dim3(nf), dim3(32), 0, st, 5, pa);
+            launches++;
+        }
+    } else {
+        if (P.corner_refine == 2) contour_refine();
+        finish(P, cam, s.d_out_count, s.d_out_ids, s.d_out_corners);
+    }
     if (refine) {  // opt-in: recover missed board markers before the stages that read the markers (fid_set_batch_marker_refinement)
         RejectedArgs ra{};
         ra.n_sel = s.d_nsel;
@@ -1149,7 +1266,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         ra.n_rej = s.d_rej_n;
         ra.rej = s.d_rej;
         launch_prio(k_rejected, dim3(nf), dim3(FINISH_THREADS), 0, st, 5, ra);
-        MarkerRefineArgs a = marker_refine_args(h, d_bgr, g.bgr_row_stride, g.bgr_frame_stride, W, H, cam);
+        MarkerRefineArgs a = marker_refine_args(h, d_bgr, g.bgr_row_stride, g.bgr_frame_stride, g.W, g.H, cam);
         a.n_rej = s.d_rej_n;
         a.rej = s.d_rej;
         a.max_rej = h->max_sel;
@@ -1208,7 +1325,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         launches++;
     }
     if (diamonds) {  // opt-in: ChArUco diamonds per frame, from the final markers (fid_set_diamonds)
-        DiamondArgs a = diamond_args(h, d_bgr, g.bgr_row_stride, g.bgr_frame_stride, W, H, cam);
+        DiamondArgs a = diamond_args(h, d_bgr, g.bgr_row_stride, g.bgr_frame_stride, g.W, g.H, cam);
         a.max_markers = h->max_markers;
         a.count = s.d_out_count;
         a.ids = s.d_out_ids;
@@ -1660,6 +1777,7 @@ extern "C" int fid_detect(fid_detector* h, const uint8_t* bgr, int width, int he
 extern "C" int fid_detect_multi_dict(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int max_markers, int* n, int32_t* ids, float* corners,
                                      int32_t* dict_indices) {
     if (!h || !n) return FID_ERR_INVALID_ARG;
+    if (h->aruco3.enable) return FID_ERR_UNSUPPORTED;  // the multi-dictionary pass is not pinned with useAruco3Detection
     int32_t count = 0;
     const int rc = detect_pose_batch(h, 1, bgr, 0, width, height, stride, stride * (size_t)height, nullptr, 0.0, 0, nullptr, nullptr, max_markers, &count, ids, corners, nullptr, false,
                                      h->multi);
@@ -1680,6 +1798,88 @@ extern "C" int fid_last_dict_indices(fid_detector* h, int max_markers, int* n_fr
     for (int f = 0; f < nf; f++)
         if (h->last_di_counts[f] > max_markers) return FID_ERR_CAPACITY;
     for (int f = 0; f < nf; f++) memcpy(out + (size_t)f * max_markers, h->last_di.data() + (size_t)f * h->last_di_stride, sizeof(int32_t) * h->last_di_counts[f]);
+    return FID_OK;
+}
+
+// Bytes of one frame's pyramid levels 1.. and segmentation plane that any frame up to max_w x max_h needs under the parameters p.
+// The levels grow with the frame.  The plane's width is round(fxfy * W') with fxfy = m / (m + max(W', H') r) <= m / (m + W' r), and
+// m W' / (m + W' r) grows with W', so max_w bounds it (+ 2 for the float32 rounding of fxfy and of the product); the same for the height.
+// With r = 0, fxfy = 1 and the gray plane serves as the segmentation plane.
+static void a3_plane_bytes(const fid_detector* h, const fid_aruco3_params& p, size_t* pyr, size_t* seg) {
+    A3Geom g;
+    a3_geometry(h->max_w, h->max_h, p.minSideLengthCanonicalImg, p.minMarkerLengthRatioOriginalImg, &g);
+    *pyr = g.pyr_frame_bytes;
+    *seg = 0;
+    if (p.minMarkerLengthRatioOriginalImg > 0) {
+        const double m = p.minSideLengthCanonicalImg, r = p.minMarkerLengthRatioOriginalImg;
+        const size_t w = std::min<size_t>(h->max_w, (size_t)(m * h->max_w / (m + h->max_w * r)) + 2);
+        const size_t ht = std::min<size_t>(h->max_h, (size_t)(m * h->max_h / (m + h->max_h * r)) + 2);
+        *seg = w * ht;
+    }
+}
+
+extern "C" int fid_set_aruco3(fid_detector* h, const fid_aruco3_params* params) {
+    if (!h || !params || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight were enqueued with the old setting
+    const fid_aruco3_params p = *params;
+    if (p.enable) {
+        if (p.minSideLengthCanonicalImg < 1 || p.minSideLengthCanonicalImg > 16384 || !(p.minMarkerLengthRatioOriginalImg >= 0.0 && p.minMarkerLengthRatioOriginalImg <= 1.0))
+            return FID_ERR_INVALID_ARG;
+        if (h->multi || h->batch_refine) return FID_ERR_UNSUPPORTED;
+        CK(cudaSetDevice(h->device));
+        size_t pyr, seg;
+        a3_plane_bytes(h, p, &pyr, &seg);
+        const size_t F = h->max_batch;
+        for (int i = 0; i < h->n_slots; i++) CK(cudaStreamSynchronize(h->slot_stream[i]));
+        CK(cudaStreamSynchronize(h->stream));
+        int rc;
+        for (int i = 0; i < h->n_slots; i++) {  // grown, never shrunk (a failed allocation leaves the mode as it was; the next enable completes it)
+            Slot& s = h->slot[i];
+            if (F * pyr > s.a3_pyr_cap) {
+                if (s.d_a3_pyr) cudaFree(s.d_a3_pyr);
+                s.d_a3_pyr = nullptr;
+                s.a3_pyr_cap = 0;
+                if ((rc = dalloc(&s.d_a3_pyr, F * pyr)) != FID_OK) return rc;
+                s.a3_pyr_cap = F * pyr;
+            }
+            if (F * seg > s.a3_seg_cap) {
+                if (s.d_a3_seg) cudaFree(s.d_a3_seg);
+                s.d_a3_seg = nullptr;
+                s.a3_seg_cap = 0;
+                if ((rc = dalloc(&s.d_a3_seg, F * seg)) != FID_OK) return rc;
+                s.a3_seg_cap = F * seg;
+            }
+        }
+    }
+    h->aruco3 = p;
+    return FID_OK;
+}
+
+extern "C" int fid_debug_aruco3_planes(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int32_t* info, uint8_t* seg, uint8_t* pyramid,
+                                       size_t pyramid_bytes) {
+    if (!h || !bgr || !info || width < 16 || height < 16 || width > h->max_w || height > h->max_h || stride < (size_t)width * h->bpp) return FID_ERR_INVALID_ARG;
+    if (h->pend_count || !h->aruco3.enable) return FID_ERR_INVALID_ARG;  // slot 0 may belong to a batch in flight
+    A3Geom ag;
+    if (!a3_geometry(width, height, h->aruco3.minSideLengthCanonicalImg, h->aruco3.minMarkerLengthRatioOriginalImg, &ag)) return FID_ERR_INVALID_ARG;
+    info[0] = ag.seg_w;
+    info[1] = ag.seg_h;
+    info[2] = ag.n_levels;
+    info[3] = ag.closest;
+    if (!seg && !pyramid) return FID_OK;  // sizes only
+    if (pyramid && pyramid_bytes < ag.pyr_frame_bytes) return FID_ERR_CAPACITY;
+    CK(cudaSetDevice(h->device));
+    Slot& s = h->slot[0];
+    CK(cudaMemcpy2DAsync(s.d_bgr, (size_t)width * h->bpp, bgr, stride, (size_t)width * h->bpp, height, cudaMemcpyHostToDevice, h->stream));
+    const FrameGeom g = make_geom(h, width, height, (size_t)width * h->bpp, (size_t)width * h->bpp * height);
+    enqueue_aruco3_planes(h, s, h->stream, 1, g, s.d_bgr, ag);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(h->stream));
+    if (seg) {
+        if (ag.resized)
+            CK(cudaMemcpy(seg, s.d_a3_seg, (size_t)ag.seg_w * ag.seg_h, cudaMemcpyDeviceToHost));
+        else
+            CK(cudaMemcpy2D(seg, width, s.d_gray, g.gray_pitch, width, height, cudaMemcpyDeviceToHost));
+    }
+    if (pyramid && ag.pyr_frame_bytes) CK(cudaMemcpy(pyramid, s.d_a3_pyr, ag.pyr_frame_bytes, cudaMemcpyDeviceToHost));
     return FID_OK;
 }
 
@@ -2059,7 +2259,7 @@ extern "C" int fid_refine_detected_markers(fid_detector* h, const uint8_t* bgr, 
 
 extern "C" int fid_set_batch_marker_refinement(fid_detector* h, int enable) {
     if (!h || h->pend_count) return FID_ERR_INVALID_ARG;
-    if (enable && h->multi) return FID_ERR_UNSUPPORTED;
+    if (enable && (h->multi || h->aruco3.enable)) return FID_ERR_UNSUPPORTED;
     if (enable) {  // (a failed allocation leaves the option off; the next enable completes it)
         CK(cudaSetDevice(h->device));
         const size_t F = h->max_batch, M = F * h->max_markers;
@@ -2360,6 +2560,7 @@ extern "C" int fid_debug_rejected(fid_detector* h, int max_rejected, int* n, flo
     if (!h || !n || max_rejected < 0 || h->pend_count) return FID_ERR_INVALID_ARG;
     if (!h->detected) return FID_ERR_INVALID_ARG;  // slot 0's candidate lists were never written
     if (h->detected_multi) return FID_ERR_UNSUPPORTED;  // detectMarkersMultiDict's rejected list (DESIGN.md finding 15) is not modelled
+    if (h->aruco3.enable) return FID_ERR_UNSUPPORTED;   // nor is the rejected list of useAruco3Detection (finding 16)
     CK(cudaSetDevice(h->device));
     int rc;
     if (!h->d_dbg_rej_n && (rc = dalloc(&h->d_dbg_rej_n, 1)) != FID_OK) return rc;

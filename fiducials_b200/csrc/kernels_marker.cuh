@@ -17,6 +17,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/fiducials_b200.h"
+#include "aruco3.cuh"
 #include "board_pnp.cuh"
 #include "candidate_tree.cuh"
 #include "charuco.cuh"
@@ -348,6 +349,7 @@ struct IdentifyArgs {
     const uint32_t* first_list;  // work list of k_identify_first (frame << 16 | k)
     uint32_t* retry_list;        // work list of k_identify_retry, filled by k_identify_first
     Counters* counters;          // n_first, n_retry
+    A3Pyramid pyr;               // useAruco3Detection (k_identify_*<true>): a candidate's bits come from its pyramid level
 };
 
 #define IDENT_WARPS 8    // retry kernel: warps per candidate
@@ -368,6 +370,33 @@ __device__ __forceinline__ void identify_write(const IdentifyArgs& a, size_t fo,
 // candidate -- every candidate of the chunk is in flight at once (a block of 8 warps per candidate held 7 idle warps' worth of
 // registers and ran the chunk in five waves).  cand_id = -2 marks the candidates whose first attempt failed and that have
 // close contours left to try.
+// PYR (useAruco3Detection, aruco3.cuh): the quads are in segmentation-plane coordinates; every attempt for a selected candidate,
+// its close contours included, reads the pyramid level its own contour length picks, with the quad scaled to that level.
+template <bool PYR>
+__device__ __forceinline__ IdentifyResult identify_attempt(const IdentifyArgs& a, const WarpLanes& L, int f, int level, const QuadF& quad, const unsigned long long* dict,
+                                                           uint8_t* img, int* hist) {
+    if constexpr (PYR) {
+        const float s = a3_level_scale(a.pyr.g, level);
+        QuadF q;
+        for (int c = 0; c < 4; c++) {
+            q.x[c] = quad.x[c] * s;
+            q.y[c] = quad.y[c] * s;
+        }
+        return identify_candidate(L, a.pyr.plane(f, level), a.pyr.g.lv[level].W, a.pyr.g.lv[level].H, q, a.P, dict, img, hist);
+    } else {
+        const FrameImg gray{a.src + (size_t)f * a.frame_stride, a.row_stride, a.enc};
+        return identify_candidate(L, gray, a.W, a.H, quad, a.P, dict, img, hist);
+    }
+}
+template <bool PYR>
+__device__ __forceinline__ int identify_level(const IdentifyArgs& a, size_t fo, int si) {
+    if constexpr (PYR)
+        return a3_level_for(a.pyr.g, a.pyr.raw[fo + a.fs.raw_of_sorted[fo + si]].n_contour);
+    else
+        return 0;
+}
+
+template <bool PYR>
 __global__ void __launch_bounds__(IDENT0_WARPS * 32) k_identify_first(const IdentifyArgs a) {
     extern __shared__ unsigned long long sm_dict[];  // n_markers*4 words, then per-warp scratch
     const unsigned int n_first = a.counters->n_first;
@@ -384,8 +413,7 @@ __global__ void __launch_bounds__(IDENT0_WARPS * 32) k_identify_first(const Iden
         const int f = (int)(rec >> 16), k = (int)(rec & 0xFFFFu);
         const size_t fo = (size_t)f * a.max_raw, o = (size_t)f * a.max_sel + k;
         const int si = a.fs.sel_idx[fo + k];
-        const FrameImg gray{a.src + (size_t)f * a.frame_stride, a.row_stride, a.enc};
-        const IdentifyResult r = identify_candidate(L, gray, a.W, a.H, a.fs.quads[fo + si], a.P, sm_dict, img, hist);
+        const IdentifyResult r = identify_attempt<PYR>(a, L, f, identify_level<PYR>(a, fo, si), a.fs.quads[fo + si], sm_dict, img, hist);
         __syncwarp();
         if (lane == 0) {
             if (r.id >= 0) {
@@ -403,6 +431,7 @@ __global__ void __launch_bounds__(IDENT0_WARPS * 32) k_identify_first(const Iden
 // One block per candidate whose first attempt failed.  A non-marker group of a dozen nested outlines used to cost a dozen
 // identifications back to back in one warp -- the longest chain of the launch.  Here warp w tries attempts 1 + w, 1 + w + 8, ...
 // concurrently; the lowest successful attempt wins, which is exactly the sequential first-success rule.
+template <bool PYR>
 __global__ void __launch_bounds__(IDENT_WARPS * 32) k_identify_retry(const IdentifyArgs a) {
     extern __shared__ unsigned long long sm_dict[];  // n_markers*4 words, then per-warp scratch
     __shared__ int s_best;                            // lowest successful attempt so far
@@ -424,12 +453,12 @@ __global__ void __launch_bounds__(IDENT_WARPS * 32) k_identify_retry(const Ident
         if (lane == 0) s_att[warp] = 0x7fffffff;
         __syncthreads();
         const int si = a.fs.sel_idx[fo + k];
-        const FrameImg gray{a.src + (size_t)f * a.frame_stride, a.row_stride, a.enc};
+        const int level = identify_level<PYR>(a, fo, si);
         const int nc = a.fs.close_count[fo + si], co = a.fs.close_off[fo + si];
         for (int t = 1 + warp; t <= nc; t += IDENT_WARPS) {
             if (t > *reinterpret_cast<volatile int*>(&s_best)) break;  // an earlier attempt already decoded
             const QuadF quad = a.fs.quads[fo + a.fs.close_idx[fo + co + t - 1]];
-            const IdentifyResult r = identify_candidate(L, gray, a.W, a.H, quad, a.P, sm_dict, img, hist);
+            const IdentifyResult r = identify_attempt<PYR>(a, L, f, level, quad, sm_dict, img, hist);
             __syncwarp();
             if (r.id >= 0) {
                 if (lane == 0) {

@@ -91,6 +91,13 @@ class FiducialsNode {
         check(fid_set_dictionaries(det, (int)all.size(), all.data()), "fid_set_dictionaries");
         specs = all;
     }
+    // Detection on a downscaled frame (new, no reference counterpart; the reference's configCallback has no such field):
+    // cv2's useAruco3Detection with minMarkerLengthRatioOriginalImg = ratio and minSideLengthCanonicalImg = min_side.  imageCallback
+    // and poseEstimateCallback then work on the full-resolution corners the mode returns.  Not with several dictionaries.
+    void setAruco3(double ratio, int min_side) {
+        const fid_aruco3_params a{1, min_side, ratio};
+        check(fid_set_aruco3(det, &a), "fid_set_aruco3");
+    }
     ~FiducialsNode() {
         if (det) fid_destroy(det);
     }

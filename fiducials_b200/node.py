@@ -185,6 +185,34 @@ class Detector:
         _lib.check(self.lib.fid_last_dict_indices(self.h, max_markers, C.byref(nf), out.ctypes.data_as(C.c_void_p)), "fid_last_dict_indices")
         return out
 
+    def set_aruco3(self, min_side: int = 32, ratio: float = 0.0, enable: bool = True):
+        """fid_set_aruco3: useAruco3Detection with minSideLengthCanonicalImg = min_side and minMarkerLengthRatioOriginalImg = ratio
+        (cv2's defaults 32 and 0); enable=False turns the mode off again."""
+        p = _lib.fid_aruco3_params(int(bool(enable)), int(min_side), float(ratio))
+        _lib.check(self.lib.fid_set_aruco3(self.h, C.byref(p)), "fid_set_aruco3")
+
+    def debug_aruco3_planes(self, bgr):
+        """fid_debug_aruco3_planes: (segmentation plane [seg_h, seg_w], [pyramid levels 1..], closest level) of one frame."""
+        bgr = np.ascontiguousarray(bgr, np.uint8)
+        H, W = bgr.shape[:2]
+        info = np.zeros(4, np.int32)
+        _lib.check(self.lib.fid_debug_aruco3_planes(self.h, bgr.ctypes.data_as(C.c_void_p), W, H, W * self.bpp, info.ctypes.data_as(C.c_void_p), None, None, 0),
+                   "fid_debug_aruco3_planes")
+        sw, sh, n_levels, closest = (int(v) for v in info)
+        sizes, w, h = [], W, H
+        for _ in range(n_levels - 1):
+            w, h = (w + 1) // 2, (h + 1) // 2
+            sizes.append((h, w))
+        seg = np.zeros((sh, sw), np.uint8)
+        pyr = np.zeros(max(1, sum(a * b for a, b in sizes)), np.uint8)
+        _lib.check(self.lib.fid_debug_aruco3_planes(self.h, bgr.ctypes.data_as(C.c_void_p), W, H, W * self.bpp, info.ctypes.data_as(C.c_void_p),
+                                                    seg.ctypes.data_as(C.c_void_p), pyr.ctypes.data_as(C.c_void_p), pyr.size), "fid_debug_aruco3_planes")
+        levels, off = [], 0
+        for h, w in sizes:
+            levels.append(pyr[off:off + h * w].reshape(h, w).copy())
+            off += h * w
+        return seg, levels, closest
+
     def set_pose_hypotheses(self, enable: bool):
         """fid_set_pose_hypotheses: batches submitted from now on also compute both planar pose solutions of every marker."""
         _lib.check(self.lib.fid_set_pose_hypotheses(self.h, int(bool(enable))), "fid_set_pose_hypotheses")
@@ -456,7 +484,7 @@ class FiducialsNode:
 
     def __init__(self, dictionary=7, fiducial_len=0.14, ignore_fiducials: Iterable[int] = (), fiducial_len_override: Optional[Dict[int, float]] = None,
                  do_pose_estimation=True, device=0, max_width=1920, max_height=1080, max_batch=1, doCornerRefinement=True, cornerRefinementSubPix=True, pose_hypotheses=False,
-                 boards=(), charuco_boards=(), refine_markers=None, diamonds=None, dictionaries=(), **detector_params):
+                 boards=(), charuco_boards=(), refine_markers=None, diamonds=None, dictionaries=(), aruco3=None, **detector_params):
         # doCornerRefinement / cornerRefinementSubPix -> cornerRefinementMethod NONE / SUBPIX / CONTOUR (:700-711, configCallback :274-281)
         if refine_markers is not None and not boards and not charuco_boards:
             raise ValueError("refine_markers needs boards or charuco_boards")
@@ -473,6 +501,10 @@ class FiducialsNode:
         if len(self.dictSpecs) > 1:
             self.det.set_dictionaries(self.dictSpecs)
         self.dictIdx = np.zeros(0, np.int32)
+        # detection on a downscaled frame (new, no reference counterpart): aruco3 = (minMarkerLengthRatioOriginalImg,
+        # minSideLengthCanonicalImg) turns on cv2's useAruco3Detection; the messages carry the full-resolution corners it returns
+        if aruco3 is not None:
+            self.det.set_aruco3(int(aruco3[1]), float(aruco3[0]))
         # both planar pose solutions of every marker (new, no reference counterpart): when on, the pose results carry an extra
         # attribute `pose_hypotheses` = {fiducial_id: fid_pose_hypotheses record}; their message fields are unchanged
         self.poseHypotheses = bool(pose_hypotheses)

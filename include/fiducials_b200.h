@@ -373,6 +373,37 @@ int fid_detect_multi_dict(fid_detector* h, const uint8_t* bgr, int width, int he
  * it.  FID_ERR_INVALID_ARG before the first batch; FID_ERR_CAPACITY, with nothing written, if a frame has more than max_markers. */
 int fid_last_dict_indices(fid_detector* h, int max_markers, int* n_frames, int32_t* out);
 
+/* Detection on a downscaled frame with pyramid corner upsampling: DetectorParameters.useAruco3Detection of OpenCV 4.13
+ * (Romero-Ramirez et al. 2018).  Off by default.  With enable set, fid_detect, fid_detect_pose_batch and fid_submit_batch /
+ * fid_collect_batch return what cv2.aruco.ArucoDetector(dictionary, params).detectMarkers returns with useAruco3Detection = True,
+ * minSideLengthCanonicalImg and minMarkerLengthRatioOriginalImg as given:
+ *   - the threshold, border-walk, quad and grouping stages run on the gray frame resized (INTER_LINEAR) by
+ *     fxfy = minSide / (minSide + max(W, H) * ratio), with a minimum contour length of 4 * minSide in place of
+ *     minMarkerPerimeterRate;
+ *   - each candidate's bits are read from the level of the frame's pyrDown pyramid that its contour length picks;
+ *   - the corners are brought back to full resolution by cornerSubPix on the pyramid levels (windows 3 and 5), whatever
+ *     cornerRefinementMethod says; with ratio 0 the frame is not scaled and no cornerSubPix runs.
+ * The pose and everything after it (pose hypotheses, boards, ChArUco, diamonds) receive the full-resolution corners and frame.
+ * Refused (FID_ERR_UNSUPPORTED, nothing changed), in both directions: several dictionaries (fid_set_dictionaries with a list that
+ * makes the handle multi-dictionary, fid_detect_multi_dict) and batch marker refinement; fid_debug_rejected refuses while the mode
+ * is on.  minSideLengthCanonicalImg 1..16384, minMarkerLengthRatioOriginalImg 0..1 (FID_ERR_INVALID_ARG otherwise).  An enable
+ * allocates each slot's pyramid and segmentation planes at the size its parameters need for frames up to fid_create's maximum (the
+ * segmentation plane is never larger than the frame, and not allocated at ratio 0), and grows them when later parameters need more.
+ * Not while batches are in flight. */
+typedef struct fid_aruco3_params {
+    int32_t enable;
+    int32_t minSideLengthCanonicalImg;       /* cv2 default 32 */
+    double minMarkerLengthRatioOriginalImg;  /* cv2 default 0 */
+} fid_aruco3_params;
+int fid_set_aruco3(fid_detector* h, const fid_aruco3_params* params);
+/* The planes the mode builds for one frame (fid_detect's arguments), for locating a mismatch: info[4] = segmentation width,
+ * height, pyramid levels (level 0 included) and the level the corners start from; seg [seg_h][seg_w] (may be NULL); pyramid: levels
+ * 1 .. n - 1 concatenated, each [h][w] with w = (w_above + 1) / 2 (may be NULL; level 0 is the gray plane of fid_debug_threshold).
+ * pyramid_bytes = the capacity of `pyramid` (FID_ERR_CAPACITY if it is too small).  With seg and pyramid both NULL only info is
+ * filled, without device work.  FID_ERR_INVALID_ARG while the mode is off. */
+int fid_debug_aruco3_planes(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int32_t* info, uint8_t* seg, uint8_t* pyramid,
+                            size_t pyramid_bytes);
+
 /* Pixel format of the frames handed to every entry point that takes `bgr` (default FID_ENC_BGR8).  The
  * reference converts whatever the camera publishes with cv_bridge::toCvCopy(msg, BGR8)
  * (aruco_detect.cpp:348) before detectMarkers turns it into gray again; the library takes the camera's own
