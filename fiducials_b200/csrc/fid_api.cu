@@ -80,6 +80,10 @@ struct Slot {
     uint8_t* d_a3_pyr = nullptr;                       // [max_batch][levels 1.. of the largest frame]
     uint8_t* d_a3_seg = nullptr;                       // [max_batch][the largest segmentation plane of the mode's parameters]
     size_t a3_pyr_cap = 0, a3_seg_cap = 0;             // their sizes in bytes; fid_set_aruco3 grows them
+    // detectMarkersWithConfidence (fid_set_marker_confidence / fid_detect_with_confidence): allocated by the first use
+    float* d_cand_conf = nullptr;                      // [max_batch][max_sel]     k_identify_*<PYR, true>
+    float* d_out_conf = nullptr;                       // [max_batch][max_markers] k_finish
+    float* h_out_conf = nullptr;
     // pinned host mirrors
     int32_t* h_out_count = nullptr;
     int32_t* h_out_ids = nullptr;
@@ -128,7 +132,7 @@ struct fid_detector {
     struct Pending {
         int first_slot, n_chunks, n_frames, w, h;
         int64_t launches;
-        bool pose, hyp, board, charuco, refine, diamonds, multi;
+        bool pose, hyp, board, charuco, refine, diamonds, multi, conf;
     } pending[MAX_SLOTS]{};
     int pend_head = 0, pend_count = 0, slots_in_use = 0, slot_next = 0;
     cudaStream_t slot_stream[MAX_SLOTS] = {};
@@ -215,6 +219,12 @@ struct fid_detector {
     int last_di_frames = 0, last_di_stride = 0;
     std::vector<int32_t> last_di_counts, last_di;    // [last_di_frames][last_di_stride]
     fid_aruco3_params aruco3{};                      // useAruco3Detection (fid_set_aruco3); enable = 0: off
+    // detectMarkersWithConfidence (fid_set_marker_confidence / fid_detect_with_confidence / fid_last_marker_confidence)
+    int marker_conf = 0;                             // the batch option
+    bool last_conf_valid = false;                    // the batch last returned had the option on
+    int last_conf_frames = 0, last_conf_stride = 0;
+    std::vector<int32_t> last_conf_counts;
+    std::vector<float> last_conf;                    // [last_conf_frames][last_conf_stride]
     bool detected_multi = false;                     // slot 0 holds fid_detect_multi_dict's candidates, not detectMarkers'
     int32_t* d_dbg_rej_n = nullptr;                  // fid_debug_rejected: count, then [max_sel][8] floats
     float* d_dbg_rej = nullptr;
@@ -329,9 +339,9 @@ static int configure_kernels(fid_detector* h) {
     CK(cudaFuncSetAttribute(k_threshold_mma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TM_SMEM_BYTES));
     CK(cudaFuncSetAttribute(k_threshold_mma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TM_SMEM_BYTES));
     CK(cudaFuncSetAttribute(k_sort_group, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)group_smem(FID_GROUP_MAX_RAW)));
-    for (auto k : {k_identify_retry<false>, k_identify_retry<true>})
+    for (auto k : {k_identify_retry<false>, k_identify_retry<true>, k_identify_retry<false, true>, k_identify_retry<true, true>})
         CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kMaxDictMarkers * 4 * 8 + IDENT_WARPS * 256 * 4 + IDENT_WARPS * FID_MAX_WARP_SIDE_SQ)));
-    for (auto k : {k_identify_first<false>, k_identify_first<true>})
+    for (auto k : {k_identify_first<false>, k_identify_first<true>, k_identify_first<false, true>, k_identify_first<true, true>})
         CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kMaxDictMarkers * 4 * 8 + IDENT0_WARPS * 256 * 4 + IDENT0_WARPS * FID_MAX_WARP_SIDE_SQ)));
     return FID_OK;
 }
@@ -407,11 +417,11 @@ static void free_slot(Slot& s) {
                      s.fs.sel_idx,    s.d_nsel,          s.d_nrawc,         s.d_cand_id,      s.d_cand_corners, s.d_out_count,    s.d_out_ids,     s.d_out_corners,
                      s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp, s.d_out_board, s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy,
                      s.d_rej_n,       s.d_rej,           s.d_mr_nrec,       s.d_mr_idx,       s.d_mr_board,    s.d_dia_n,       s.d_dia,
-                     s.d_md_count,    s.d_md_ids,        s.d_md_corners,    s.d_out_dict,     s.d_a3_pyr,      s.d_a3_seg};
+                     s.d_md_count,    s.d_md_ids,        s.d_md_corners,    s.d_out_dict,     s.d_a3_pyr,      s.d_a3_seg,      s.d_cand_conf,   s.d_out_conf};
     for (void* p : dptrs)
         if (p) cudaFree(p);
     void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp, s.h_out_board, s.h_out_ch, s.h_out_ch_ids, s.h_out_ch_xy,
-                     s.h_rej_n,     s.h_rej,     s.h_mr_nrec,    s.h_mr_idx,   s.h_mr_board, s.h_dia_n, s.h_dia, s.h_out_dict};
+                     s.h_rej_n,     s.h_rej,     s.h_mr_nrec,    s.h_mr_idx,   s.h_mr_board, s.h_dia_n, s.h_dia, s.h_out_dict, s.h_out_conf};
     for (void* p : hptrs)
         if (p) cudaFreeHost(p);
     for (int i = 0; i <= ST_COUNT; i++)
@@ -635,7 +645,7 @@ extern "C" int fid_set_dictionaries(fid_detector* h, int n, const fid_dictionary
         if ((int64_t)specs[d].id_offset + dp[d].n_markers - 1 > INT32_MAX) return FID_ERR_INVALID_ARG;  // a published id would overflow
     }
     const bool multi = n > 1 || specs[0].id_offset != 0 || specs[0].fiducial_len > 0;
-    if (multi && (h->n_boards || h->n_charuco || h->batch_refine || h->diamond.enable || h->aruco3.enable)) return FID_ERR_UNSUPPORTED;
+    if (multi && (h->n_boards || h->n_charuco || h->batch_refine || h->diamond.enable || h->aruco3.enable || h->marker_conf)) return FID_ERR_UNSUPPORTED;
     CK(cudaSetDevice(h->device));
     if (multi) {  // (a failed allocation leaves the handle as it was; the next call completes it)
         const size_t F = h->max_batch, M = F * h->max_markers, ND = FID_MAX_DICTIONARIES;
@@ -872,7 +882,7 @@ static int enqueue_aruco3_planes(const fid_detector* h, Slot& s, cudaStream_t st
 
 static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, const FrameGeom& g, const uint8_t* d_bgr, const fid_camera* cam, double fiducial_len,
                             int n_override, int stop_after /* -1 = all */, const Slot* prev = nullptr, bool refine = false, bool diamonds = false,
-                            bool multi = false) {
+                            bool multi = false, bool conf = false) {
     const DevParams& P = h->P;
     int launches = 0;
     CK(cudaMemsetAsync(s.d_counters, 0, sizeof(Counters), st));
@@ -1115,8 +1125,12 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.retry_list = s.d_retry_list;
         a.counters = s.d_counters;
         // fixed grids over work lists: a grid of one block per (frame, candidate slot) is 32 768 blocks of which 1 500 have work
-        if (a3) {
-            a.pyr = A3Pyramid{s.d_gray, g.gray_frame_stride, s.d_a3_pyr, s.d_raw, ag};
+        if (a3) a.pyr = A3Pyramid{s.d_gray, g.gray_frame_stride, s.d_a3_pyr, s.d_raw, ag};
+        if (conf) {  // detectMarkersWithConfidence
+            a.cand_conf = s.d_cand_conf;
+            launch_prio(a3 ? k_identify_first<true, true> : k_identify_first<false, true>, dim3(h->sm_count * 4), dim3(IDENT0_WARPS * 32), ident_smem(Pd, IDENT0_WARPS), st, 4, a);
+            launch_prio(a3 ? k_identify_retry<true, true> : k_identify_retry<false, true>, dim3(h->sm_count * 2), dim3(IDENT_WARPS * 32), ident_smem(Pd, IDENT_WARPS), st, 4, a);
+        } else if (a3) {
             launch_prio(k_identify_first<true>, dim3(h->sm_count * 4), dim3(IDENT0_WARPS * 32), ident_smem(Pd, IDENT0_WARPS), st, 4, a);
             launch_prio(k_identify_retry<true>, dim3(h->sm_count * 2), dim3(IDENT_WARPS * 32), ident_smem(Pd, IDENT_WARPS), st, 4, a);
         } else {
@@ -1168,6 +1182,19 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.counters = s.d_counters;
         launch_prio(k_finish, dim3(nf), dim3(FINISH_THREADS), 0, st, 5, a);
         launches++;
+        if (conf) {  // detectMarkersWithConfidence: the candidates' confidences in marker order
+            ConfGatherArgs ca{};
+            ca.n_sel = s.d_nsel;
+            ca.cand_id = s.d_cand_id;
+            ca.cand_conf = s.d_cand_conf;
+            ca.fs = s.fs;
+            ca.max_raw = h->max_raw;
+            ca.max_sel = h->max_sel;
+            ca.max_markers = h->max_markers;
+            ca.out_conf = s.d_out_conf;
+            launch_prio(k_conf_gather, dim3(nf), dim3(FINISH_THREADS), 0, st, 5, ca);
+            launches++;
+        }
     };
     if (multi) {  // several dictionaries (fid_set_dictionaries): the front end above ran once
         const size_t F = h->max_batch, dstride = F * h->max_markers;
@@ -1342,8 +1369,9 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
 }
 
 static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool with_pose, bool with_hyp, bool with_board, bool with_charuco, bool with_refine,
-                       bool with_diamonds, bool multi = false) {
+                       bool with_diamonds, bool multi = false, bool with_conf = false) {
     const size_t M = (size_t)nf * h->max_markers;
+    if (with_conf) CK(cudaMemcpyAsync(s.h_out_conf, s.d_out_conf, sizeof(float) * M, cudaMemcpyDeviceToHost, st));
     if (multi) CK(cudaMemcpyAsync(s.h_out_dict, s.d_out_dict, sizeof(int32_t) * M, cudaMemcpyDeviceToHost, st));
     if (with_diamonds) CK(cudaMemcpyAsync(s.h_dia_n, s.d_dia_n, sizeof(int32_t) * nf, cudaMemcpyDeviceToHost, st));  // collect copies the records
     if (with_refine) {  // counts only: collect copies the lists at their lengths
@@ -1371,7 +1399,7 @@ static int enqueue_d2h(fid_detector* h, Slot& s, cudaStream_t st, int nf, bool w
 
 static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* tfs, bool first_chunk,
                    struct fid_pose_hypotheses* hyps = nullptr, fid_board_pose* boards = nullptr, int ch_first = -1, bool refined = false, bool diamonds = false,
-                   int32_t* dict_idx = nullptr, bool multi = false) {
+                   int32_t* dict_idx = nullptr, bool multi = false, float* conf = nullptr) {
     CK(cudaEventSynchronize(s.done));
     int status = FID_OK;
     if (diamonds) {  // the diamond records (fid_last_diamonds), each row at the frame with the most diamonds
@@ -1424,6 +1452,7 @@ static int collect(fid_detector* h, Slot& s, int nf, int max_markers, int32_t* c
         if (hyps) memcpy(hyps + (size_t)f * max_markers, s.h_out_hyp + (size_t)f * h->max_markers, sizeof(struct fid_pose_hypotheses) * n);
         if (dict_idx && multi) memcpy(dict_idx + (size_t)f * max_markers, s.h_out_dict + (size_t)f * h->max_markers, sizeof(int32_t) * n);
         if (dict_idx && !multi) memset(dict_idx + (size_t)f * max_markers, 0, sizeof(int32_t) * n);
+        if (conf) memcpy(conf + (size_t)f * max_markers, s.h_out_conf + (size_t)f * h->max_markers, sizeof(float) * n);
     }
     if (boards) memcpy(boards, s.h_out_board, sizeof(fid_board_pose) * nf * h->n_boards);
     if (ch_first >= 0) {  // frames ch_first .. of the ChArUco records of the batch (fid_last_charuco)
@@ -1502,6 +1531,21 @@ static void end_last_dict_indices(fid_detector* h, const int32_t* counts) {
     h->last_di_valid = true;
 }
 
+// The same for the marker confidences (fid_last_marker_confidence).
+static float* begin_last_confidence(fid_detector* h, bool conf, int n_frames, int max_markers) {
+    h->last_conf_valid = false;
+    if (!conf) return nullptr;
+    h->last_conf_frames = n_frames;
+    h->last_conf_stride = max_markers;
+    h->last_conf.resize((size_t)n_frames * max_markers);
+    return h->last_conf.data();
+}
+static void end_last_confidence(fid_detector* h, bool conf, const int32_t* counts) {
+    if (!conf) return;
+    h->last_conf_counts.assign(counts, counts + h->last_conf_frames);
+    h->last_conf_valid = true;
+}
+
 // The same for the board poses (fid_last_board_poses), dense [n_frames][n_boards].
 static fid_board_pose* begin_last_boards(fid_detector* h, bool board, int n_frames) {
     h->last_board_valid = false;
@@ -1548,7 +1592,7 @@ static void begin_last_diamonds(fid_detector* h, bool dia, int n_frames) {
 // fid_detect_pose_batch; fid_detect (detectMarkers) passes may_refine = false, which also leaves diamonds out.
 static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
                              const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
-                             int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms, bool may_refine, bool multi) {
+                             int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms, bool may_refine, bool multi, bool conf) {
     if (!h || !bgr || !counts || n_frames < 0 || width < 16 || height < 16 || width > h->max_w || height > h->max_h || max_markers < 0) return FID_ERR_INVALID_ARG;
     if (row_stride < (size_t)width * h->bpp || frame_stride < row_stride * (size_t)height) return FID_ERR_INVALID_ARG;
     if (cam && !(fiducial_len > 0)) return FID_ERR_INVALID_ARG;
@@ -1572,6 +1616,7 @@ static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, 
     const bool dia = may_refine && h->diamond.enable;
     begin_last_diamonds(h, dia, n_frames);
     int32_t* dict_idx = begin_last_dict_indices(h, n_frames, max_markers);
+    float* confs = begin_last_confidence(h, conf, n_frames, max_markers);
     h->counters[6] = 0;
     h->stage_ms[ST_H2D] = 0;
     // software pipeline over chunks: up to n_slots chunks in flight, each on its own stream; results of
@@ -1622,9 +1667,9 @@ static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, 
                 h->pf_h = height;
                 h->hint_next = nullptr;
             }
-            rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, c > 0 ? &h->slot[(c - 1) % NS] : nullptr, mr, dia, multi);
+            rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, c > 0 ? &h->slot[(c - 1) % NS] : nullptr, mr, dia, multi, conf);
             if (rc != FID_OK) return rc;
-            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp, brd, chr, mr, dia, multi);
+            rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, hyp, brd, chr, mr, dia, multi, conf);
             if (rc != FID_OK) return rc;
             h->last_frames = nf;
         }
@@ -1635,12 +1680,13 @@ static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, 
             rc = collect(h, s, nf, max_markers, counts + (size_t)pc * B, ids ? ids + (size_t)pc * B * max_markers : nullptr,
                          corners ? corners + (size_t)pc * B * max_markers * 8 : nullptr, (transforms && cam) ? transforms + (size_t)pc * B * max_markers : nullptr, pc == 0,
                          hyps ? hyps + (size_t)pc * B * max_markers : nullptr, boards ? boards + (size_t)pc * B * h->n_boards : nullptr, chr ? pc * B : -1, mr, dia,
-                         dict_idx + (size_t)pc * B * max_markers, multi);
+                         dict_idx + (size_t)pc * B * max_markers, multi, confs ? confs + (size_t)pc * B * max_markers : nullptr);
             if (rc != FID_OK) status = rc;
         }
     }
     end_last_hypotheses(h, hyp, counts);
     end_last_dict_indices(h, counts);
+    end_last_confidence(h, conf, counts);
     h->last_board_valid = brd;
     h->last_ch_valid = chr;
     h->last_mr_valid = mr;
@@ -1652,7 +1698,7 @@ extern "C" int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_
                                      const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
                                      int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms) {
     return detect_pose_batch(h, n_frames, bgr, bgr_on_device, width, height, row_stride, frame_stride, cam, fiducial_len, n_override, override_ids, override_lens,
-                             max_markers, counts, ids, corners, transforms, true, h && h->multi);
+                             max_markers, counts, ids, corners, transforms, true, h && h->multi, h && h->marker_conf);
 }
 
 extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
@@ -1700,9 +1746,9 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
             g = make_geom(h, width, height, (size_t)width * h->bpp, (size_t)width * h->bpp * height);
         }
         const Slot* prev = (h->slots_in_use + c) > 0 ? &h->slot[(si + NS - 1) % NS] : nullptr;
-        rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, prev, mr, dia, h->multi);
+        rc = enqueue_pipeline(h, s, cst, nf, g, d_in, cam, fiducial_len, n_override, -1, prev, mr, dia, h->multi, h->marker_conf != 0);
         if (rc != FID_OK) return rc;
-        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam, h->n_boards && cam, h->n_charuco > 0, mr, dia, h->multi);
+        rc = enqueue_d2h(h, s, cst, nf, cam != nullptr, h->pose_hyp && cam, h->n_boards && cam, h->n_charuco > 0, mr, dia, h->multi, h->marker_conf != 0);
         if (rc != FID_OK) return rc;
         h->last_frames = nf;
     }
@@ -1719,6 +1765,7 @@ extern "C" int fid_submit_batch(fid_detector* h, int n_frames, const uint8_t* bg
     pb.refine = mr;
     pb.diamonds = dia;
     pb.multi = h->multi;
+    pb.conf = h->marker_conf != 0;
     pb.launches = h->counters[6];
     h->pend_count++;
     h->slots_in_use += n_chunks;
@@ -1740,17 +1787,20 @@ extern "C" int fid_collect_batch(fid_detector* h, int max_markers, int32_t* coun
     begin_last_refinement(h, pb.refine, pb.n_frames);
     begin_last_diamonds(h, pb.diamonds, pb.n_frames);
     int32_t* dict_idx = begin_last_dict_indices(h, pb.n_frames, max_markers);
+    float* confs = begin_last_confidence(h, pb.conf, pb.n_frames, max_markers);
     for (int c = 0; c < pb.n_chunks; c++) {
         Slot& s = h->slot[(pb.first_slot + c) % NS];
         const int nf = std::min(B, pb.n_frames - c * B);
         const int rc = collect(h, s, nf, max_markers, counts + (size_t)c * B, ids ? ids + (size_t)c * B * max_markers : nullptr,
                                corners ? corners + (size_t)c * B * max_markers * 8 : nullptr, (transforms && pb.pose) ? transforms + (size_t)c * B * max_markers : nullptr, c == 0,
                                hyps ? hyps + (size_t)c * B * max_markers : nullptr, boards ? boards + (size_t)c * B * h->n_boards : nullptr,
-                               pb.charuco ? c * B : -1, pb.refine, pb.diamonds, dict_idx + (size_t)c * B * max_markers, pb.multi);
+                               pb.charuco ? c * B : -1, pb.refine, pb.diamonds, dict_idx + (size_t)c * B * max_markers, pb.multi,
+                               confs ? confs + (size_t)c * B * max_markers : nullptr);
         if (rc != FID_OK) status = rc;
     }
     end_last_hypotheses(h, pb.hyp, counts);
     end_last_dict_indices(h, counts);
+    end_last_confidence(h, pb.conf, counts);
     h->last_board_valid = pb.board;
     h->last_ch_valid = pb.charuco;
     h->last_mr_valid = pb.refine;
@@ -1765,7 +1815,7 @@ extern "C" int fid_detect(fid_detector* h, const uint8_t* bgr, int width, int he
     if (!n) return FID_ERR_INVALID_ARG;
     int32_t count = 0;
     const int rc = detect_pose_batch(h, 1, bgr, 0, width, height, stride, stride * (size_t)height, nullptr, 0.0, 0, nullptr, nullptr, max_markers, &count, ids, corners, nullptr, false,
-                                     false);
+                                     false, false);
     if (rc == FID_OK || rc == FID_ERR_CAPACITY) {
         h->detected = true;
         h->detected_multi = false;
@@ -1780,7 +1830,7 @@ extern "C" int fid_detect_multi_dict(fid_detector* h, const uint8_t* bgr, int wi
     if (h->aruco3.enable) return FID_ERR_UNSUPPORTED;  // the multi-dictionary pass is not pinned with useAruco3Detection
     int32_t count = 0;
     const int rc = detect_pose_batch(h, 1, bgr, 0, width, height, stride, stride * (size_t)height, nullptr, 0.0, 0, nullptr, nullptr, max_markers, &count, ids, corners, nullptr, false,
-                                     h->multi);
+                                     h->multi, false);
     if (rc == FID_OK || rc == FID_ERR_CAPACITY) {
         h->detected = true;
         h->detected_multi = h->multi;
@@ -1798,6 +1848,61 @@ extern "C" int fid_last_dict_indices(fid_detector* h, int max_markers, int* n_fr
     for (int f = 0; f < nf; f++)
         if (h->last_di_counts[f] > max_markers) return FID_ERR_CAPACITY;
     for (int f = 0; f < nf; f++) memcpy(out + (size_t)f * max_markers, h->last_di.data() + (size_t)f * h->last_di_stride, sizeof(int32_t) * h->last_di_counts[f]);
+    return FID_OK;
+}
+
+// Each slot's confidence buffers, allocated by the first use (a failed allocation leaves them for the next use to complete).
+static int alloc_confidence(fid_detector* h) {
+    CK(cudaSetDevice(h->device));
+    const size_t F = h->max_batch, M = F * h->max_markers;
+    for (int i = 0; i < h->n_slots; i++) {
+        Slot& s = h->slot[i];
+        int rc;
+        if (!s.d_cand_conf && (rc = dalloc(&s.d_cand_conf, F * h->max_sel)) != FID_OK) return rc;
+        if (!s.d_out_conf && (rc = dalloc(&s.d_out_conf, M)) != FID_OK) return rc;
+        if (!s.h_out_conf && (rc = halloc(&s.h_out_conf, M)) != FID_OK) return rc;
+    }
+    return FID_OK;
+}
+
+extern "C" int fid_detect_with_confidence(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int max_markers, int* n, int32_t* ids, float* corners,
+                                          float* confidence) {
+    if (!h || !n) return FID_ERR_INVALID_ARG;
+    if (h->multi) return FID_ERR_UNSUPPORTED;  // cv2 has no confidence for detectMarkersMultiDict
+    if (h->pend_count) return FID_ERR_INVALID_ARG;
+    int rc = alloc_confidence(h);
+    if (rc != FID_OK) return rc;
+    int32_t count = 0;
+    rc = detect_pose_batch(h, 1, bgr, 0, width, height, stride, stride * (size_t)height, nullptr, 0.0, 0, nullptr, nullptr, max_markers, &count, ids, corners, nullptr, false, false,
+                           true);
+    if (rc == FID_OK || rc == FID_ERR_CAPACITY) {
+        h->detected = true;
+        h->detected_multi = false;
+        if (confidence) memcpy(confidence, h->last_conf.data(), sizeof(float) * count);
+    }
+    *n = count;
+    return rc;
+}
+
+extern "C" int fid_set_marker_confidence(fid_detector* h, int enable) {
+    if (!h || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight were enqueued with the old setting
+    if (enable && (h->multi || h->batch_refine)) return FID_ERR_UNSUPPORTED;  // neither detectMarkersMultiDict nor recovered markers have a confidence
+    if (enable) {
+        const int rc = alloc_confidence(h);
+        if (rc != FID_OK) return rc;
+    }
+    h->marker_conf = enable ? 1 : 0;
+    return FID_OK;
+}
+
+extern "C" int fid_last_marker_confidence(fid_detector* h, int max_markers, int* n_frames, float* out) {
+    if (!h || !n_frames || max_markers < 0 || !h->last_conf_valid) return FID_ERR_INVALID_ARG;
+    const int nf = h->last_conf_frames;
+    *n_frames = nf;
+    if (!out) return FID_OK;
+    for (int f = 0; f < nf; f++)
+        if (h->last_conf_counts[f] > max_markers) return FID_ERR_CAPACITY;
+    for (int f = 0; f < nf; f++) memcpy(out + (size_t)f * max_markers, h->last_conf.data() + (size_t)f * h->last_conf_stride, sizeof(float) * h->last_conf_counts[f]);
     return FID_OK;
 }
 
@@ -2259,7 +2364,7 @@ extern "C" int fid_refine_detected_markers(fid_detector* h, const uint8_t* bgr, 
 
 extern "C" int fid_set_batch_marker_refinement(fid_detector* h, int enable) {
     if (!h || h->pend_count) return FID_ERR_INVALID_ARG;
-    if (enable && (h->multi || h->aruco3.enable)) return FID_ERR_UNSUPPORTED;
+    if (enable && (h->multi || h->aruco3.enable || h->marker_conf)) return FID_ERR_UNSUPPORTED;
     if (enable) {  // (a failed allocation leaves the option off; the next enable completes it)
         CK(cudaSetDevice(h->device));
         const size_t F = h->max_batch, M = F * h->max_markers;

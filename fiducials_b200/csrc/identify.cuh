@@ -164,7 +164,9 @@ struct CellBits {
 // _extractBits: perspective removal (nearest warp), Otsu or the minOtsuStdDev rule, cell votes.  ok = false where the quad
 // gives no perspective transform.  Returned by value: through an out pointer k_identify_first spilled more.
 // `img` : S*S bytes of scratch, `hist`: 256 ints of scratch (zeroed by this function).
-template <class Lanes, class Img>
+// CONF (detectMarkersWithConfidence): where ok, hist[c] holds on return cell c's count of window pixels above the threshold --
+// the whole window (win^2) or none in the minOtsuStdDev rule, as the bits there.
+template <bool CONF = false, class Lanes, class Img>
 FID_HD CellBits extract_bits(const Lanes& L, const Img& gray, int W, int H, const QuadF& quad, const DevParams& P, uint8_t* img, int* hist) {
     CellBits out = {0ull, 0ull, false};
     const int cells = P.marker_size + 2 * P.marker_border_bits;
@@ -201,15 +203,23 @@ FID_HD CellBits extract_bits(const Lanes& L, const Img& gray, int W, int H, cons
     unsigned long long bits_lo = 0, bits_hi = 0;
     if (stddev < P.min_otsu_stddev) {
         if (mean > 127.0) bits_lo = bits_hi = ~0ull;  // all white (bits beyond cells*cells are never read)
+        if constexpr (CONF) {
+            const int win = cell - 2 * margin;
+            L.sync();  // every lane is done with the histogram
+            for (int c = L.lane(); c < cells * cells; c += L.count()) hist[c] = mean > 127.0 ? win * win : 0;
+            L.sync();
+        }
     } else {
         const int t = otsu_threshold(hist, S * S);
         const int win = cell - 2 * margin;
+        if constexpr (CONF) L.sync();  // every lane has read the histogram
         unsigned long long mine = 0, mine_hi = 0;
         for (int c = L.lane(); c < cells * cells; c += L.count()) {
             const int cy = c / cells, cx = c - cy * cells;
             int nz = 0;
             for (int yy = 0; yy < win; yy++)
                 for (int xx = 0; xx < win; xx++) nz += img[(cy * cell + margin + yy) * S + cx * cell + margin + xx] > t ? 1 : 0;
+            if constexpr (CONF) hist[c] = nz;
             if (nz > (win * win) / 2) {
                 if (c < 64)
                     mine |= 1ull << c;
@@ -219,6 +229,7 @@ FID_HD CellBits extract_bits(const Lanes& L, const Img& gray, int W, int H, cons
         }
         bits_lo = L.or_u64(mine);
         bits_hi = cells * cells > 64 ? L.or_u64(mine_hi) : 0ull;
+        if constexpr (CONF) L.sync();
     }
     out.lo = bits_lo;
     out.hi = bits_hi;
@@ -249,13 +260,42 @@ FID_HD unsigned long long inner_code(const CellBits& b, const DevParams& P) {
     return cand;
 }
 
+// detectMarkersWithConfidence (DESIGN.md finding 17): 1 - the mean over the cells of the share of each cell's window that
+// disagrees with the decoded marker -- black in the border, inside the dictionary word `word` as identify_candidate matched it
+// (the rotation seen in the canonical image).  Not the extracted bits: an inner cell that error correction fixed costs its
+// whole share.  cnt = extract_bits<true>'s counts.  Each cell's share is a float; their sum is exact in double (81 floats in
+// [0, 1] whose exponents span less than 53 bits) and rounded once to float before the float division: independent of the order,
+// so the kernels and the host agree bit for bit.  cv2's own order is not pinned; where win^2 is not a power of two the two can
+// differ in the last float bit.
+FID_HD float marker_confidence(const int* cnt, const DevParams& P, unsigned long long word) {
+    const int bb = P.marker_border_bits, ms = P.marker_size, cells = ms + 2 * bb;
+    const int margin = (int)(P.ignored_margin_per_cell * P.px_per_cell);
+    const int win = P.px_per_cell - 2 * margin;
+    const float area = (float)(win * win);
+    const int total = ms * ms, last_byte = (total - 1) >> 3, last_bits = total & 7 ? total & 7 : 8;
+    double sum = 0.0;
+    for (int y = 0; y < cells; y++)
+        for (int x = 0; x < cells; x++) {
+            const float ratio = (float)cnt[y * cells + x] / area;
+            bool one = false;
+            if (y >= bb && y < cells - bb && x >= bb && x < cells - bb) {  // inner_code's packing: row-major, MSB first per byte
+                const int k = (y - bb) * ms + x - bb, byte = k >> 3;
+                const int nb = byte == last_byte ? last_bits : 8;
+                one = (word >> (8 * byte + nb - 1 - (k & 7))) & 1ull;
+            }
+            sum += one ? 1.0f - ratio : ratio;
+        }
+    return 1.0f - (float)sum / (float)(cells * cells);
+}
+
 // `img` : S*S bytes of scratch, `hist`: 256 ints of scratch (zeroed by this function).
 // dict  : n_markers x 4 rotations packed as little-endian byte strings in 64-bit words.
-template <class Lanes, class Img>
+// CONF: on a match hist holds the cell counts marker_confidence reads, with word dict[id * 4 + rotation].
+template <bool CONF = false, class Lanes, class Img>
 FID_HD IdentifyResult identify_candidate(const Lanes& L, const Img& gray, int W, int H, const QuadF& quad, const DevParams& P, const unsigned long long* dict, uint8_t* img,
                                          int* hist) {
     IdentifyResult res = {-1, 0};
-    const CellBits bits = extract_bits(L, gray, W, H, quad, P, img, hist);
+    const CellBits bits = extract_bits<CONF>(L, gray, W, H, quad, P, img, hist);
     if (!bits.ok) return res;
     // border errors (_getBorderErrors) -- number of white bits in the border ring
     const int cells = P.marker_size + 2 * P.marker_border_bits;

@@ -350,6 +350,7 @@ struct IdentifyArgs {
     uint32_t* retry_list;        // work list of k_identify_retry, filled by k_identify_first
     Counters* counters;          // n_first, n_retry
     A3Pyramid pyr;               // useAruco3Detection (k_identify_*<true>): a candidate's bits come from its pyramid level
+    float* cand_conf;            // [F][max_sel] detectMarkersWithConfidence (k_identify_*<PYR, true>), decoded candidates only
 };
 
 #define IDENT_WARPS 8    // retry kernel: warps per candidate
@@ -372,7 +373,9 @@ __device__ __forceinline__ void identify_write(const IdentifyArgs& a, size_t fo,
 // close contours left to try.
 // PYR (useAruco3Detection, aruco3.cuh): the quads are in segmentation-plane coordinates; every attempt for a selected candidate,
 // its close contours included, reads the pyramid level its own contour length picks, with the quad scaled to that level.
-template <bool PYR>
+// CONF (detectMarkersWithConfidence): each decoded candidate's confidence goes to cand_conf, from the cell counts the attempt
+// that decoded left in its warp's `hist` (identify.cuh, marker_confidence).
+template <bool PYR, bool CONF>
 __device__ __forceinline__ IdentifyResult identify_attempt(const IdentifyArgs& a, const WarpLanes& L, int f, int level, const QuadF& quad, const unsigned long long* dict,
                                                            uint8_t* img, int* hist) {
     if constexpr (PYR) {
@@ -382,10 +385,10 @@ __device__ __forceinline__ IdentifyResult identify_attempt(const IdentifyArgs& a
             q.x[c] = quad.x[c] * s;
             q.y[c] = quad.y[c] * s;
         }
-        return identify_candidate(L, a.pyr.plane(f, level), a.pyr.g.lv[level].W, a.pyr.g.lv[level].H, q, a.P, dict, img, hist);
+        return identify_candidate<CONF>(L, a.pyr.plane(f, level), a.pyr.g.lv[level].W, a.pyr.g.lv[level].H, q, a.P, dict, img, hist);
     } else {
         const FrameImg gray{a.src + (size_t)f * a.frame_stride, a.row_stride, a.enc};
-        return identify_candidate(L, gray, a.W, a.H, quad, a.P, dict, img, hist);
+        return identify_candidate<CONF>(L, gray, a.W, a.H, quad, a.P, dict, img, hist);
     }
 }
 template <bool PYR>
@@ -396,7 +399,7 @@ __device__ __forceinline__ int identify_level(const IdentifyArgs& a, size_t fo, 
         return 0;
 }
 
-template <bool PYR>
+template <bool PYR, bool CONF = false>
 __global__ void __launch_bounds__(IDENT0_WARPS * 32) k_identify_first(const IdentifyArgs a) {
     extern __shared__ unsigned long long sm_dict[];  // n_markers*4 words, then per-warp scratch
     const unsigned int n_first = a.counters->n_first;
@@ -413,11 +416,12 @@ __global__ void __launch_bounds__(IDENT0_WARPS * 32) k_identify_first(const Iden
         const int f = (int)(rec >> 16), k = (int)(rec & 0xFFFFu);
         const size_t fo = (size_t)f * a.max_raw, o = (size_t)f * a.max_sel + k;
         const int si = a.fs.sel_idx[fo + k];
-        const IdentifyResult r = identify_attempt<PYR>(a, L, f, identify_level<PYR>(a, fo, si), a.fs.quads[fo + si], sm_dict, img, hist);
+        const IdentifyResult r = identify_attempt<PYR, CONF>(a, L, f, identify_level<PYR>(a, fo, si), a.fs.quads[fo + si], sm_dict, img, hist);
         __syncwarp();
         if (lane == 0) {
             if (r.id >= 0) {
                 identify_write(a, fo, o, r.id, r.rotation, si);
+                if constexpr (CONF) a.cand_conf[o] = marker_confidence(hist, a.P, sm_dict[r.id * 4 + r.rotation]);
             } else if (a.fs.close_count[fo + si] > 0) {
                 a.cand_id[o] = -2;
                 a.retry_list[atomicAdd(&a.counters->n_retry, 1u)] = rec;
@@ -425,13 +429,14 @@ __global__ void __launch_bounds__(IDENT0_WARPS * 32) k_identify_first(const Iden
                 a.cand_id[o] = -1;
             }
         }
+        if constexpr (CONF) __syncwarp();  // lane 0 is done with the counts before the next candidate overwrites them
     }
 }
 
 // One block per candidate whose first attempt failed.  A non-marker group of a dozen nested outlines used to cost a dozen
 // identifications back to back in one warp -- the longest chain of the launch.  Here warp w tries attempts 1 + w, 1 + w + 8, ...
 // concurrently; the lowest successful attempt wins, which is exactly the sequential first-success rule.
-template <bool PYR>
+template <bool PYR, bool CONF = false>
 __global__ void __launch_bounds__(IDENT_WARPS * 32) k_identify_retry(const IdentifyArgs a) {
     extern __shared__ unsigned long long sm_dict[];  // n_markers*4 words, then per-warp scratch
     __shared__ int s_best;                            // lowest successful attempt so far
@@ -458,7 +463,7 @@ __global__ void __launch_bounds__(IDENT_WARPS * 32) k_identify_retry(const Ident
         for (int t = 1 + warp; t <= nc; t += IDENT_WARPS) {
             if (t > *reinterpret_cast<volatile int*>(&s_best)) break;  // an earlier attempt already decoded
             const QuadF quad = a.fs.quads[fo + a.fs.close_idx[fo + co + t - 1]];
-            const IdentifyResult r = identify_attempt<PYR>(a, L, f, level, quad, sm_dict, img, hist);
+            const IdentifyResult r = identify_attempt<PYR, CONF>(a, L, f, level, quad, sm_dict, img, hist);
             __syncwarp();
             if (r.id >= 0) {
                 if (lane == 0) {
@@ -472,16 +477,19 @@ __global__ void __launch_bounds__(IDENT_WARPS * 32) k_identify_retry(const Ident
         }
         __syncthreads();
         if (threadIdx.x == 0) {
-            int id = -1, rot = 0, att = 0;
+            int id = -1, rot = 0, att = 0, win_w = 0;
             for (int w = 0; w < IDENT_WARPS; w++)
                 if (s_att[w] == s_best && s_best != 0x7fffffff) {
                     id = s_id[w];
                     rot = s_rot[w];
                     att = s_att[w];
+                    if constexpr (CONF) win_w = w;
                 }
-            if (id >= 0)
+            if (id >= 0) {
                 identify_write(a, fo, o, id, rot, a.fs.close_idx[fo + co + att - 1]);
-            else
+                // the winning warp stopped after its decoding attempt: its hist still holds that attempt's counts
+                if constexpr (CONF) a.cand_conf[o] = marker_confidence(reinterpret_cast<int*>(sm_dict + n_words) + win_w * 256, a.P, sm_dict[id * 4 + rot]);
+            } else
                 a.cand_id[o] = -1;
         }
     }
@@ -761,6 +769,41 @@ __global__ void __launch_bounds__(FINISH_THREADS) k_finish(const FinishArgs a) {
 // detectMarkers' rejectedImgPoints (DESIGN.md finding 11): the selected candidates that are not markers -- not decoded, or decoded
 // on a level of the candidate hierarchy that identification never reached -- in selection order (descending perimeter), each with
 // the selected quad's own corners (integers, clockwise, neither rotated nor refined).  One block per frame, after k_finish.
+// detectMarkersWithConfidence (fid_set_marker_confidence / fid_detect_with_confidence): the confidences k_identify_*<PYR, true>
+// wrote per candidate, in k_finish's marker order -- the decoded candidates on a level identification reached, in selection order,
+// at most max_markers.  The hierarchy is restated through candidate_tree.cuh as k_rejected does, so that k_finish stays as it is.
+// One block per frame, after k_finish.
+struct ConfGatherArgs {
+    const int* n_sel;
+    const int* cand_id;
+    const float* cand_conf;  // [F][max_sel]
+    FrameScratch fs;
+    int max_raw, max_sel, max_markers;
+    float* out_conf;         // [F][max_markers]
+};
+
+__global__ void __launch_bounds__(FINISH_THREADS) k_conf_gather(const ConfGatherArgs a) {
+    __shared__ short s_parent[FID_MAX_SEL], s_depth[FID_MAX_SEL];
+    __shared__ unsigned char s_was[FID_MAX_SEL];
+    const int f = blockIdx.x, tid = threadIdx.x;
+    const int ns = a.n_sel[f] < FID_MAX_SEL ? a.n_sel[f] : FID_MAX_SEL;
+    const size_t fo = (size_t)f * a.max_raw;
+    const int* cand_id = a.cand_id + (size_t)f * a.max_sel;
+    for (int i = tid; i < ns; i += FINISH_THREADS) {
+        s_parent[i] = (short)tree_parent(a.fs.quads[fo + a.fs.sel_idx[fo + i]], i, [&](int j) { return a.fs.quads[fo + a.fs.sel_idx[fo + j]]; });
+        s_depth[i] = 0;
+        s_was[i] = 0;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        tree_levels(ns, s_parent, s_depth, s_was, [&](int v) { return cand_id[v] >= 0; });
+        const int cap = a.max_markers < FID_MAX_MARKERS ? a.max_markers : FID_MAX_MARKERS;
+        int n = 0;
+        for (int k = 0; k < ns && n < cap; k++)
+            if (cand_id[k] >= 0 && (s_was[k] & 2)) a.out_conf[(size_t)f * a.max_markers + n++] = a.cand_conf[(size_t)f * a.max_sel + k];
+    }
+}
+
 struct RejectedArgs {
     const int* n_sel;
     const int* cand_id;

@@ -185,6 +185,30 @@ class Detector:
         _lib.check(self.lib.fid_last_dict_indices(self.h, max_markers, C.byref(nf), out.ctypes.data_as(C.c_void_p)), "fid_last_dict_indices")
         return out
 
+    def detect_with_confidence(self, bgr: np.ndarray):
+        """fid_detect_with_confidence (detectMarkersWithConfidence): (ids int32[n], corners float32[n,4,2], confidence float32[n])."""
+        bgr = np.ascontiguousarray(bgr, np.uint8)
+        H, W = bgr.shape[:2]
+        ids = np.zeros(MAXM, np.int32)
+        corners = np.zeros((MAXM, 8), np.float32)
+        conf = np.zeros(MAXM, np.float32)
+        n = C.c_int(0)
+        _lib.check(self.lib.fid_detect_with_confidence(self.h, bgr.ctypes.data_as(C.c_void_p), W, H, W * self.bpp, MAXM, C.byref(n), ids.ctypes.data_as(C.c_void_p),
+                                                       corners.ctypes.data_as(C.c_void_p), conf.ctypes.data_as(C.c_void_p)), "fid_detect_with_confidence")
+        return ids[: n.value].copy(), corners[: n.value].reshape(-1, 4, 2).copy(), conf[: n.value].copy()
+
+    def set_marker_confidence(self, enable: bool):
+        """fid_set_marker_confidence: batches submitted from now on also compute every marker's detection confidence."""
+        _lib.check(self.lib.fid_set_marker_confidence(self.h, int(bool(enable))), "fid_set_marker_confidence")
+
+    def last_marker_confidence(self, max_markers=MAXM):
+        """fid_last_marker_confidence: float32 [n_frames, max_markers], laid out like the ids of the batch last returned."""
+        nf = C.c_int(0)
+        _lib.check(self.lib.fid_last_marker_confidence(self.h, max_markers, C.byref(nf), None), "fid_last_marker_confidence")
+        out = np.zeros((nf.value, max_markers), np.float32)
+        _lib.check(self.lib.fid_last_marker_confidence(self.h, max_markers, C.byref(nf), out.ctypes.data_as(C.c_void_p)), "fid_last_marker_confidence")
+        return out
+
     def set_aruco3(self, min_side: int = 32, ratio: float = 0.0, enable: bool = True):
         """fid_set_aruco3: useAruco3Detection with minSideLengthCanonicalImg = min_side and minMarkerLengthRatioOriginalImg = ratio
         (cv2's defaults 32 and 0); enable=False turns the mode off again."""

@@ -404,6 +404,27 @@ int fid_set_aruco3(fid_detector* h, const fid_aruco3_params* params);
 int fid_debug_aruco3_planes(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int32_t* info, uint8_t* seg, uint8_t* pyramid,
                             size_t pyramid_bytes);
 
+/* Per-marker detection confidence: cv2.aruco.ArucoDetector.detectMarkersWithConfidence of OpenCV 4.13.  A marker's confidence is
+ * 1 - the mean over its cells of the share of each cell's sampling window that disagrees with the decoded marker (black border,
+ * the dictionary word of the id inside), on the canonical image identification reads: 1.0 for a clean marker, lower for cells
+ * that error correction fixed, partial occlusion or glare.  float32, computed at identification (whatever
+ * cornerRefinementMethod says; on the pyramid level with useAruco3Detection).
+ * fid_detect_with_confidence: one frame (fid_detect's arguments); ids and corners exactly as fid_detect returns them, and
+ * confidence[n] (may be NULL).  Works whether or not the batch option is on.  FID_ERR_UNSUPPORTED in multi-dictionary mode (cv2
+ * has no confidence for detectMarkersMultiDict). */
+int fid_detect_with_confidence(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int max_markers, int* n, int32_t* ids, float* corners,
+                               float* confidence);
+/* Opt-in confidence of the batch calls (default off): with it on, fid_detect_pose_batch and fid_submit_batch / fid_collect_batch
+ * also compute every marker's confidence; ids, corners and transforms are unchanged.  Refused (FID_ERR_UNSUPPORTED, nothing
+ * changed), in both directions: several dictionaries (fid_set_dictionaries) and batch marker refinement (recovered markers have no
+ * cv2 confidence).  Not while batches are in flight.  The first use allocates the result buffers. */
+int fid_set_marker_confidence(fid_detector* h, int enable);
+/* Confidences of the batch most recently returned by fid_collect_batch / fid_detect_pose_batch (or fid_detect_with_confidence),
+ * dense [n_frames][max_markers] in the marker order of that batch (entries past counts[f] are not written).  *n_frames = the
+ * batch's frame count; out may be NULL to query it.  FID_ERR_INVALID_ARG if the option was off for that batch; FID_ERR_CAPACITY,
+ * with nothing written, if a frame of the batch has more markers than max_markers. */
+int fid_last_marker_confidence(fid_detector* h, int max_markers, int* n_frames, float* out);
+
 /* Pixel format of the frames handed to every entry point that takes `bgr` (default FID_ENC_BGR8).  The
  * reference converts whatever the camera publishes with cv_bridge::toCvCopy(msg, BGR8)
  * (aruco_detect.cpp:348) before detectMarkers turns it into gray again; the library takes the camera's own
