@@ -290,42 +290,132 @@ FID_HD int walk_resume_bidir(const WalkCtx& c, int x0, int y0, int max_len, int 
 }
 
 // ---- hot-loop versions ----------------------------------------------------------------------------------
-// Same walks on packed pixels (y << 16 | x: raster order is unsigned integer order, a move is one add of
-// the table's packed delta) with 32-bit index arithmetic and the per-step max_len test hoisted out of the
-// loop.  A warp executes its instruction stream in order, so the length of the longest walk of a launch
-// times the instructions per step IS the tail latency of the launch: these loops are written for
-// instruction count.  Results are identical to walk_resume_dir / walk_resume_bidir
-// (tests/test_hostsim_contours.py).
-FID_HD uint32_t idx9_packed(const uint32_t* plane, uint32_t tiles_per_row, uint32_t xy) {
-    const uint32_t x = xy & 0xFFFFu, y = xy >> 16;
-    const uint32_t qx = (x * 34953u) >> 20, qy = (y * 34953u) >> 20;
-    const uint32_t i = x - FID_HALO_T * qx;
-    const uint32_t* t = plane + ((qy * tiles_per_row + qx) * 32u + (y - FID_HALO_T * qy));
-    return ((t[0] >> i) & 7u) | (((t[1] >> i) & 7u) << 3) | (((t[2] >> i) & 7u) << 6);
+// Same walks on packed pixels (y << 16 | x: raster order is unsigned integer order) with the per-step max_len
+// test hoisted out of the loop.  The lanes of a warp sit on unrelated borders, so every global load of a step is
+// a 128-byte transaction of its own per active lane; the loops keep those few:
+//  * a walker keeps the three tile words around its pixel in registers (TileWin).  A step moves one pixel: a
+//    horizontal move loads nothing, a vertical or diagonal one loads one word, and only a move out of the
+//    30 x 30 tile loads three (from the neighbouring tile, whose halo again holds the whole neighbourhood);
+//  * the loops read bits 0-4 of a step-table entry (direction, crack flags) through step_load() and derive the
+//    move from the direction, so that the kernels can walk on byte-per-entry copies of the tables in shared
+//    memory (StepTabs<uint8_t>) while the WalkCtx overloads below read the 32-bit tables.
+// What this buys on the H100 is in DESIGN.md section 4 ("What a walk step costs").
+// Results are identical to walk_resume_dir / walk_resume_bidir (tests/test_hostsim_contours.py,
+// tests/test_hostsim_walk_window.py).
+template <class E>
+struct StepTabs {
+    const E* prev;
+    const E* next;
+};
+FID_HD uint32_t step_load(const uint32_t* p) { return lut_load(p) & 31u; }
+FID_HD uint32_t step_load(const uint8_t* p) { return *p; }
+inline void build_step_bytes(uint8_t* prev, uint8_t* next) {
+    uint32_t p[FID_LUT_SIZE], n[FID_LUT_SIZE];
+    build_step_tables(p, n);
+    for (int k = 0; k < FID_LUT_SIZE; k++) {
+        prev[k] = (uint8_t)(p[k] & 31u);
+        next[k] = (uint8_t)(n[k] & 31u);
+    }
 }
-FID_HD uint32_t entry_of_dir(int dir) { return (uint32_t)dir | (pack_move(dir) << 5); }
-#define FID_MOVE(xy, e) ((xy) + ((e) >> 5) - 65537u)
 
-// One-directional walk of at most `budget` steps (round 0).
-template <bool IS_RIGHT>
-FID_HD int walk_uni_fast(const WalkCtx& c, int x0, int y0, int max_len, int budget, WalkState* st) {
-    const uint32_t* plane = c.plane.base;
-    const uint32_t tpr = (uint32_t)c.plane.tiles_per_row;
-    const uint32_t* lut = IS_RIGHT ? c.lut_next : c.lut_prev;
+struct TileWin {
+    uint32_t o;           // word offset of the walker's tile in the plane
+    int r, i;             // the pixel is bit i + 1 of word r + 1 of that tile, 0 <= r, i < FID_HALO_T
+    uint32_t w0, w1, w2;  // words r, r + 1, r + 2
+    FID_HD void load(const uint32_t* plane) {
+        const uint32_t* t = plane + o + r;
+        w0 = t[0];
+        w1 = t[1];
+        w2 = t[2];
+    }
+    FID_HD void enter(const uint32_t* plane, uint32_t tiles_per_row, uint32_t xy) {
+        const uint32_t x = xy & 0xFFFFu, y = xy >> 16;
+        const uint32_t qx = (x * 34953u) >> 20, qy = (y * 34953u) >> 20;
+        o = (qy * tiles_per_row + qx) * 32u;
+        r = (int)(y - FID_HALO_T * qy);
+        i = (int)(x - FID_HALO_T * qx);
+        load(plane);
+    }
+    // from a tile index and the word / bit of the pixel inside the tile (1 .. FID_HALO_T: what a start record holds)
+    FID_HD void enter_tile(const uint32_t* plane, uint32_t tile, uint32_t row, uint32_t col) {
+        o = tile * 32u;
+        r = (int)row - 1;
+        i = (int)col - 1;
+        load(plane);
+    }
+    FID_HD uint32_t idx9() const { return ((w0 >> i) & 7u) | (((w1 >> i) & 7u) << 3) | (((w2 >> i) & 7u) << 6); }
+    // Move by (dx, dy), each in -1 .. 1, to a pixel inside the image.
+    FID_HD void step(const uint32_t* plane, uint32_t tiles_per_row, int dx, int dy) {
+        i += dx;
+        r += dy;
+        if ((unsigned)i >= (unsigned)FID_HALO_T || (unsigned)r >= (unsigned)FID_HALO_T) {
+            if (i < 0) {
+                i = FID_HALO_T - 1;
+                o -= 32u;
+            } else if (i >= FID_HALO_T) {
+                i = 0;
+                o += 32u;
+            }
+            if (r < 0) {
+                r = FID_HALO_T - 1;
+                o -= tiles_per_row * 32u;
+            } else if (r >= FID_HALO_T) {
+                r = 0;
+                o += tiles_per_row * 32u;
+            }
+            load(plane);
+        } else if (dy != 0) {
+            const uint32_t nw = plane[o + (uint32_t)(r + 1 + dy)];
+            const uint32_t mid = dy > 0 ? w2 : w0;
+            w0 = dy > 0 ? w1 : nw;
+            w2 = dy > 0 ? nw : w1;
+            w1 = mid;
+        }
+    }
+};
+FID_HD uint32_t move_of(int dx, int dy) { return (uint32_t)(dy * 65536 + dx); }
+
+// walk_init on a neighbourhood already read (v = idx9 of the start pixel).
+template <class E>
+FID_HD int walk_init_at(uint32_t v, const StepTabs<E>& tabs, int x0, int y0, int is_right, WalkState* st) {
+    if ((v & ~0x10u) == 0u) return WALK_ABORT;
+    const int crack = is_right ? 0 : 4;
+    const int a0 = (int)(step_load(tabs.prev + v * 8 + crack) & 7u);
+    const int b0 = (int)(step_load(tabs.next + v * 8 + crack) & 7u);
+    if (is_right) {
+        const int d = (b0 - a0 - 1) & 7;
+        if (((4 - a0 - 1) & 7) < d) return WALK_ABORT;
+    }
+    st->x = x0;
+    st->y = y0;
+    st->n = 0;
+    st->a0 = a0;
+    st->b0 = b0;
+    st->dir = is_right ? b0 : a0;
+    return WALK_CONTINUE;
+}
+
+// One-directional walk of at most `budget` steps (round 0).  `w` sits on the walker's pixel (st->x, st->y) and
+// follows it; lut = the table of the walk's direction (IS_RIGHT ? next : prev).
+template <bool IS_RIGHT, class E>
+FID_HD int walk_uni_fast(const uint32_t* plane, uint32_t tpr, const E* lut, TileWin& w, int x0, int y0, int max_len, int budget, WalkState* st) {
     const uint32_t xy0 = (uint32_t)x0 | ((uint32_t)y0 << 16);
     const uint32_t ref = (uint32_t)(IS_RIGHT ? st->a0 : st->b0);
     uint32_t xy = (uint32_t)st->x | ((uint32_t)st->y << 16);
-    uint32_t e = entry_of_dir(st->dir);
+    uint32_t d = (uint32_t)st->dir;
     int result = WALK_CONTINUE, k = 0;
     for (; k < budget; k++) {
-        xy = FID_MOVE(xy, e);
-        const uint32_t back = (e & 7u) ^ 4u;
+        const int dx = dir_dx((int)d), dy = dir_dy((int)d);
+        xy += move_of(dx, dy);
+        const uint32_t back = d ^ 4u;
         if (xy == xy0 && back == ref) {
             result = WALK_CANONICAL;
             k++;
             break;
         }
-        e = lut_load(lut + idx9_packed(plane, tpr, xy) * 8u + back);
+        w.step(plane, tpr, dx, dy);
+        const uint32_t e = step_load(lut + w.idx9() * 8u + back);
+        d = e & 7u;
         if ((e & 0x18u) && (xy < xy0 || (IS_RIGHT && (e & 8u) && xy == xy0))) {
             result = WALK_ABORT;
             k++;
@@ -334,48 +424,57 @@ FID_HD int walk_uni_fast(const WalkCtx& c, int x0, int y0, int max_len, int budg
     }
     st->x = (int)(xy & 0xFFFFu);
     st->y = (int)(xy >> 16);
-    st->dir = (int)(e & 7u);
+    st->dir = (int)d;
     st->n += k;
     if (st->n > max_len && result != WALK_ABORT) result = WALK_TOO_LONG;
     return result;
 }
-
-// Bidirectional walk of at most `budget` steps (budget/2 lock-step iterations).
 template <bool IS_RIGHT>
-FID_HD int walk_bidir_fast(const WalkCtx& c, int x0, int y0, int max_len, int budget, WalkState2* st) {
-    const uint32_t* plane = c.plane.base;
+FID_HD int walk_uni_fast(const WalkCtx& c, int x0, int y0, int max_len, int budget, WalkState* st) {
     const uint32_t tpr = (uint32_t)c.plane.tiles_per_row;
+    TileWin w;
+    w.enter(c.plane.base, tpr, (uint32_t)st->x | ((uint32_t)st->y << 16));
+    return walk_uni_fast<IS_RIGHT>(c.plane.base, tpr, IS_RIGHT ? c.lut_next : c.lut_prev, w, x0, y0, max_len, budget, st);
+}
+
+// Bidirectional walk of at most `budget` steps (budget/2 lock-step iterations).  wf / wb sit on the forward and
+// the backward walker's pixel and follow them while the walk continues.
+template <bool IS_RIGHT, class E>
+FID_HD int walk_bidir_fast(const uint32_t* plane, uint32_t tpr, const StepTabs<E>& tabs, TileWin& wf, TileWin& wb, int x0, int y0, int max_len, int budget,
+                           WalkState2* st) {
     const uint32_t xy0 = (uint32_t)x0 | ((uint32_t)y0 << 16);
     uint32_t xyf = (uint32_t)st->xf | ((uint32_t)st->yf << 16), xyb = (uint32_t)st->xb | ((uint32_t)st->yb << 16);
-    uint32_t ef = entry_of_dir(st->df), eb = entry_of_dir(st->db);
+    uint32_t df = (uint32_t)st->df, db = (uint32_t)st->db;
     const int iters = (budget + 1) >> 1;
     int result = WALK_CONTINUE, it = 0, half = 0;
     for (; it < iters; it++) {
         // both moves and both table look-ups first (two independent chains), then the tests in walk order
-        const uint32_t xyf1 = FID_MOVE(xyf, ef), xyb1 = FID_MOVE(xyb, eb);
-        const uint32_t back_f = (ef & 7u) ^ 4u, back_b = (eb & 7u) ^ 4u;
-        const uint32_t ef1 = lut_load(c.lut_next + idx9_packed(plane, tpr, xyf1) * 8u + back_f);
-        const uint32_t eb1 = lut_load(c.lut_prev + idx9_packed(plane, tpr, xyb1) * 8u + back_b);
-        const uint32_t db = eb & 7u;
+        const int dxf = dir_dx((int)df), dyf = dir_dy((int)df), dxb = dir_dx((int)db), dyb = dir_dy((int)db);
+        const uint32_t xyf1 = xyf + move_of(dxf, dyf), xyb1 = xyb + move_of(dxb, dyb);
+        const uint32_t back_f = df ^ 4u, back_b = db ^ 4u;
+        wf.step(plane, tpr, dxf, dyf);
+        wb.step(plane, tpr, dxb, dyb);
+        const uint32_t ef1 = step_load(tabs.next + wf.idx9() * 8u + back_f);
+        const uint32_t eb1 = step_load(tabs.prev + wb.idx9() * 8u + back_b);
         xyf = xyf1;
         if (xyf1 == xyb && back_f == db) {  // the forward walker arrived on the backward walker's state
             result = WALK_CANONICAL;
             half = 1;
             break;
         }
-        ef = ef1;
+        df = ef1 & 7u;
         if ((ef1 & 0x18u) && (xyf1 < xy0 || (IS_RIGHT && (ef1 & 8u) && xyf1 == xy0))) {
             result = WALK_ABORT;
             half = 1;
             break;
         }
         xyb = xyb1;
-        if (xyb1 == xyf1 && back_b == (ef1 & 7u)) {  // the backward walker arrived on the forward walker's new state
+        if (xyb1 == xyf1 && back_b == df) {  // the backward walker arrived on the forward walker's new state
             result = WALK_CANONICAL;
             half = 2;
             break;
         }
-        eb = eb1;
+        db = eb1 & 7u;
         if ((eb1 & 0x18u) && (xyb1 < xy0 || (IS_RIGHT && (eb1 & 8u) && xyb1 == xy0))) {
             result = WALK_ABORT;
             half = 2;
@@ -384,14 +483,22 @@ FID_HD int walk_bidir_fast(const WalkCtx& c, int x0, int y0, int max_len, int bu
     }
     st->xf = (int)(xyf & 0xFFFFu);
     st->yf = (int)(xyf >> 16);
-    st->df = (int)(ef & 7u);
+    st->df = (int)df;
     st->xb = (int)(xyb & 0xFFFFu);
     st->yb = (int)(xyb >> 16);
-    st->db = (int)(eb & 7u);
+    st->db = (int)db;
     st->n += 2 * it + half;
     st->nf += it + (half ? 1 : 0);
     if (st->n > max_len && result != WALK_ABORT) result = WALK_TOO_LONG;
     return result;
+}
+template <bool IS_RIGHT>
+FID_HD int walk_bidir_fast(const WalkCtx& c, int x0, int y0, int max_len, int budget, WalkState2* st) {
+    const uint32_t tpr = (uint32_t)c.plane.tiles_per_row;
+    TileWin wf, wb;
+    wf.enter(c.plane.base, tpr, (uint32_t)st->xf | ((uint32_t)st->yf << 16));
+    wb.enter(c.plane.base, tpr, (uint32_t)st->xb | ((uint32_t)st->yb << 16));
+    return walk_bidir_fast<IS_RIGHT>(c.plane.base, tpr, StepTabs<uint32_t>{c.lut_prev, c.lut_next}, wf, wb, x0, y0, max_len, budget, st);
 }
 
 FID_HD int walk_resume(const WalkCtx& c, int x0, int y0, int is_right, int max_len, int budget, WalkState* st) {
@@ -466,25 +573,59 @@ struct WalkCkpt {
 
 // forward: points[off + t] = pixel after t steps, t = 0 .. count-1
 // backward: points[off - t] = pixel after t steps, t = 1 .. count
-FID_HD void trace_segment(const WalkCtx& c, const SegRec& s, uint32_t* points) {
-    const uint32_t* plane = c.plane.base;
-    const uint32_t tpr = (uint32_t)c.plane.tiles_per_row;
-    uint32_t xy = s.xy, e = entry_of_dir((int)(s.dn & 7));
+// Points are written in ascending-address groups of four words that start at a multiple of four (one 16-byte
+// store each; `points` is 16-byte aligned), single words before the first and after the last full group of
+// the segment: a segment never writes a word that is not its own.
+FID_HD void store_points4(uint32_t* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+#if defined(__CUDA_ARCH__)
+    *reinterpret_cast<uint4*>(p) = make_uint4(a, b, c, d);
+#else
+    p[0] = a;
+    p[1] = b;
+    p[2] = c;
+    p[3] = d;
+#endif
+}
+template <class E>
+FID_HD void trace_segment(const uint32_t* plane, uint32_t tpr, const StepTabs<E>& tabs, const SegRec& s, uint32_t* points) {
+    const bool backward = (s.meta & 1u) != 0u;
+    const E* lut = backward ? tabs.prev : tabs.next;
     const int count = (int)(s.dn >> 3);
-    uint32_t* out = points + s.off;
-    if (s.meta & 1u) {
-        for (int t = 1; t <= count; t++) {
-            xy = FID_MOVE(xy, e);
-            out[-t] = xy;
-            e = lut_load(c.lut_prev + idx9_packed(plane, tpr, xy) * 8u + ((e & 7u) ^ 4u));
+    uint32_t xy = s.xy, d = s.dn & 7u;
+    TileWin w;
+    w.enter(plane, tpr, xy);
+    // the walker's next point: a forward segment starts with the state's own pixel, a backward one with the first move
+    auto next_point = [&]() {
+        const int dx = dir_dx((int)d), dy = dir_dy((int)d);
+        const uint32_t cur = xy;
+        xy += move_of(dx, dy);
+        w.step(plane, tpr, dx, dy);
+        d = step_load(lut + w.idx9() * 8u + (d ^ 4u)) & 7u;
+        return backward ? xy : cur;
+    };
+    int t = 0;
+    if (backward) {  // words off-1, off-2, ..., off-count
+        uint32_t at = s.off;  // one past the next word to write
+        for (; t < count && (at & 3u); t++) points[--at] = next_point();
+        for (; t + 4 <= count; t += 4) {
+            const uint32_t p3 = next_point(), p2 = next_point(), p1 = next_point(), p0 = next_point();
+            at -= 4;
+            store_points4(points + at, p0, p1, p2, p3);
         }
-    } else {
-        for (int t = 0; t < count; t++) {
-            out[t] = xy;
-            xy = FID_MOVE(xy, e);
-            e = lut_load(c.lut_next + idx9_packed(plane, tpr, xy) * 8u + ((e & 7u) ^ 4u));
+        for (; t < count; t++) points[--at] = next_point();
+    } else {  // words off, off+1, ..., off+count-1
+        uint32_t at = s.off;
+        for (; t < count && (at & 3u); t++) points[at++] = next_point();
+        for (; t + 4 <= count; t += 4) {
+            const uint32_t p0 = next_point(), p1 = next_point(), p2 = next_point(), p3 = next_point();
+            store_points4(points + at, p0, p1, p2, p3);
+            at += 4;
         }
+        for (; t < count; t++) points[at++] = next_point();
     }
+}
+FID_HD void trace_segment(const WalkCtx& c, const SegRec& s, uint32_t* points) {
+    trace_segment(c.plane.base, (uint32_t)c.plane.tiles_per_row, StepTabs<uint32_t>{c.lut_prev, c.lut_next}, s, points);
 }
 
 // Number of segments of a contour, and the segments themselves (sink(k, SegRec) for k = 0 .. count-1).

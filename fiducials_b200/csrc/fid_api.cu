@@ -149,6 +149,7 @@ struct fid_detector {
     int start_prune = 0;
     uint32_t* d_lut_prev = nullptr;
     uint32_t* d_lut_next = nullptr;
+    uint8_t* d_step_bytes = nullptr;  // bits 0-4 of both step tables, a byte per entry (k_walk / k_emit stage them into shared memory)
     int thresh_mode = 0;  // 0 = summed-area-table kernel (kernels_threshold.cuh, default: faster end to end), 1 = tensor-core kernel (kernels_threshold_mma.cuh; FID_THRESH=mma)
     int walk_rounds = 0;
     int walk_refill = 16, walk_pass = 16;  // persistent rounds: idle lanes that trigger a refill, steps per pass (FID_WALK_REFILL / FID_WALK_PASS)
@@ -520,6 +521,13 @@ extern "C" int fid_create(const fid_params* params, int device, int max_width, i
         }
         CKH(cudaMemcpy(h->d_lut_prev, lp.data(), FID_LUT_SIZE * sizeof(uint32_t), cudaMemcpyHostToDevice));
         CKH(cudaMemcpy(h->d_lut_next, ln.data(), FID_LUT_SIZE * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        std::vector<uint8_t> sb(2 * FID_LUT_SIZE);
+        build_step_bytes(sb.data(), sb.data() + FID_LUT_SIZE);
+        if ((rc = dalloc(&h->d_step_bytes, sb.size())) != FID_OK) {
+            fid_destroy(h);
+            return rc;
+        }
+        CKH(cudaMemcpy(h->d_step_bytes, sb.data(), sb.size(), cudaMemcpyHostToDevice));
     }
     {   // walk plan: budgets per round, 'p' prefix = persistent lanes, 0 = unbounded (must be last)
         if (const char* e = getenv("FID_EMIT_BLOCKS")) h->emit_blocks_per_sm = std::max(1, atoi(e));
@@ -573,7 +581,7 @@ extern "C" int fid_destroy(fid_detector* h) {
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();
     for (int i = 0; i < MAX_SLOTS; i++) free_slot(h->slot[i]);
-    void* ptrs[] = {h->d_prune, h->d_dict, h->d_pf[0], h->d_pf[1], h->d_lut_prev, h->d_lut_next, h->d_subpix_masks, h->d_override_ids, h->d_override_lens, h->d_pose_ids, h->d_pose_corners, h->d_pose_out, h->d_hyp_list,
+    void* ptrs[] = {h->d_prune, h->d_dict, h->d_pf[0], h->d_pf[1], h->d_lut_prev, h->d_lut_next, h->d_step_bytes, h->d_subpix_masks, h->d_override_ids, h->d_override_lens, h->d_pose_ids, h->d_pose_corners, h->d_pose_out, h->d_hyp_list,
                      h->d_board_off, h->d_board_keys, h->d_board_marker, h->d_board_obj, h->d_board_count, h->d_board_list, h->d_ch_boards, h->d_ch_keys,
                      h->d_ch_marker, h->d_ch_ids, h->d_ch_near_n, h->d_ch_near_idx, h->d_ch_near_corner, h->d_ch_obj, h->d_ch_chess, h->d_ch_masks,
                      h->d_ch_count, h->d_ch_list, h->d_ch_list_ids, h->d_ch_list_xy, h->d_mr_i, h->d_mr_f, h->d_dbg_rej_n, h->d_dbg_rej, h->d_dia_io, h->d_dia_list, h->d_mdict};
@@ -1012,6 +1020,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.halo = s.d_halo;
         a.lut_prev = h->d_lut_prev;
         a.lut_next = h->d_lut_next;
+        a.step_bytes = h->d_step_bytes;
         a.starts = s.d_starts;
         a.chains = s.d_chains;
         a.segs = s.d_segs;
@@ -1046,8 +1055,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
     {  // emit
         EmitArgs a{};
         a.halo = s.d_halo;
-        a.lut_prev = h->d_lut_prev;
-        a.lut_next = h->d_lut_next;
+        a.step_bytes = h->d_step_bytes;
         a.segs = s.d_segs;
         a.points = s.d_points;
         a.counters = s.d_counters;

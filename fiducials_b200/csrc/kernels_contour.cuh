@@ -68,8 +68,8 @@ struct FrameGeom {
     uint32_t magic_tpr, magic_tiles_y;  // ceil(2^32 / d): __umulhi(t, magic) == t / d for t < 2^18, d < 2^14
 };
 
-// start record -> (pixel, meta = frame << 8 | scale << 1 | is_right)
-__device__ __forceinline__ void start_rec_unpack(const FrameGeom& g, uint32_t v, uint32_t is_right, uint32_t* xy, uint32_t* meta) {
+// start record -> (pixel, meta = frame << 8 | scale << 1 | is_right, index of its tile in its plane)
+__device__ __forceinline__ void start_rec_unpack(const FrameGeom& g, uint32_t v, uint32_t is_right, uint32_t* xy, uint32_t* meta, uint32_t* plane_tile) {
     const uint32_t tile = v >> 14, scale = (v >> 10) & 15u, row = (v >> 5) & 31u, col = v & 31u;
     const uint32_t trow = __umulhi(tile, g.magic_tpr);            // f * tiles_y + ty
     const uint32_t tx = tile - trow * (uint32_t)g.halo_tpr;
@@ -77,6 +77,17 @@ __device__ __forceinline__ void start_rec_unpack(const FrameGeom& g, uint32_t v,
     const uint32_t ty = trow - f * (uint32_t)g.halo_tiles_y;
     *xy = (FID_HALO_T * tx - 1u + col) | ((FID_HALO_T * ty - 1u + row) << 16);
     *meta = (f << 8) | (scale << 1) | is_right;
+    *plane_tile = ty * (uint32_t)g.halo_tpr + tx;
+}
+
+// Byte-per-entry copies of the two step tables (prev, then next) in a block's shared memory: a table look-up of
+// the walk's hot loops is then a shared-memory read and not one more 128-byte global transaction per lane.
+__device__ __forceinline__ StepTabs<uint8_t> stage_step_tables(const uint8_t* step_bytes, uint8_t* smem) {
+    const uint4* src = reinterpret_cast<const uint4*>(step_bytes);
+    uint4* dst = reinterpret_cast<uint4*>(smem);
+    for (unsigned int k = threadIdx.x; k < 2u * FID_LUT_SIZE / 16u; k += blockDim.x) dst[k] = __ldg(src + k);
+    __syncthreads();
+    return StepTabs<uint8_t>{smem, smem + FID_LUT_SIZE};
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -93,6 +104,7 @@ struct WalkArgs {
     const uint32_t* halo;
     const uint32_t* lut_prev;
     const uint32_t* lut_next;
+    const uint8_t* step_bytes;  // bits 0-4 of lut_prev's, then of lut_next's entries (build_step_bytes)
     const StartRec* starts;   // round 0 input: left items at [0, nL), right items at [max_starts-1 ...]
     const WalkRec* q_in;      // later rounds: left items at [0, nL), right items at [max_queue-1 ...]
     WalkRec* q_out;
@@ -114,6 +126,7 @@ struct WalkItem {
     WalkState2 st;
     int x0, y0;
     WalkCtx ctx;
+    TileWin wf, wb;  // the two walkers' tile words, kept across the passes of a round
 };
 
 __device__ __forceinline__ WalkCtx walk_ctx_of(const WalkArgs& a, uint32_t meta) {
@@ -142,6 +155,8 @@ __device__ __forceinline__ void walk_load_item(const WalkArgs& a, unsigned int i
     it.x0 = it.xy0 & 0xFFFF;
     it.y0 = it.xy0 >> 16;
     it.ctx = walk_ctx_of(a, it.meta);
+    it.wf.enter(it.ctx.plane.base, (uint32_t)a.g.halo_tpr, w1.x);
+    it.wb.enter(it.ctx.plane.base, (uint32_t)a.g.halo_tpr, w1.y);
 }
 
 template <bool IS_RIGHT>
@@ -179,7 +194,7 @@ __device__ __forceinline__ void walk_retire(const WalkArgs& a, int result, uint3
 }
 
 template <bool IS_RIGHT>
-__device__ __forceinline__ void walk_side(const WalkArgs& a, unsigned int n, unsigned int first_warp, unsigned int n_warps) {
+__device__ __forceinline__ void walk_side(const WalkArgs& a, const StepTabs<uint8_t>& tabs, unsigned int n, unsigned int first_warp, unsigned int n_warps) {
     // `n` items of one direction, processed by warps first_warp .. first_warp+n_warps-1 of the grid
     const unsigned int lane = threadIdx.x & 31;
     const unsigned int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -191,15 +206,17 @@ __device__ __forceinline__ void walk_side(const WalkArgs& a, unsigned int n, uns
         for (unsigned int base = my * 32; base < n; base += n_warps * 32) {
             const unsigned int idx = base + lane;
             if (idx >= n) continue;
-            uint32_t sxy, smeta;
+            uint32_t sxy, smeta, stile;
             const uint32_t srec = a.starts[IS_RIGHT ? a.max_starts - 1 - idx : idx].v;
             if (srec == FID_START_NULL) continue;
-            start_rec_unpack(a.g, srec, IS_RIGHT ? 1u : 0u, &sxy, &smeta);
+            start_rec_unpack(a.g, srec, IS_RIGHT ? 1u : 0u, &sxy, &smeta, &stile);
             const WalkCtx ctx = walk_ctx_of(a, smeta);
             const int x0 = sxy & 0xFFFF, y0 = sxy >> 16;
+            TileWin w;
+            w.enter_tile(ctx.plane.base, stile, (srec >> 5) & 31u, srec & 31u);
             WalkState st;
-            if (walk_init(ctx, x0, y0, IS_RIGHT ? 1 : 0, &st) != WALK_CONTINUE) continue;
-            const int r = walk_uni_fast<IS_RIGHT>(ctx, x0, y0, a.max_len, a.budget, &st);
+            if (walk_init_at(w.idx9(), tabs, x0, y0, IS_RIGHT ? 1 : 0, &st) != WALK_CONTINUE) continue;
+            const int r = walk_uni_fast<IS_RIGHT>(ctx.plane.base, (uint32_t)a.g.halo_tpr, IS_RIGHT ? tabs.next : tabs.prev, w, x0, y0, a.max_len, a.budget, &st);
             WalkState2 s2;
             walk_split<IS_RIGHT>(x0, y0, st, &s2);
             walk_retire<IS_RIGHT>(a, r, sxy, smeta, s2, ctx, nullptr);
@@ -212,7 +229,7 @@ __device__ __forceinline__ void walk_side(const WalkArgs& a, unsigned int n, uns
             if (idx >= n) continue;
             WalkItem it;
             walk_load_item<IS_RIGHT>(a, idx, it);
-            const int r = walk_bidir_fast<IS_RIGHT>(it.ctx, it.x0, it.y0, a.max_len, a.budget, &it.st);
+            const int r = walk_bidir_fast<IS_RIGHT>(it.ctx.plane.base, (uint32_t)a.g.halo_tpr, tabs, it.wf, it.wb, it.x0, it.y0, a.max_len, a.budget, &it.st);
             walk_retire<IS_RIGHT>(a, r, it.xy0, it.meta, it.st, it.ctx, nullptr);
         }
         return;
@@ -262,7 +279,8 @@ __device__ __forceinline__ void walk_side(const WalkArgs& a, unsigned int n, uns
         }
         if (active) {
             const int left = budget_end - it.st.n;
-            const int r = walk_bidir_fast<IS_RIGHT>(it.ctx, it.x0, it.y0, a.max_len, left < a.pass_steps ? left : a.pass_steps, &it.st);
+            const int r = walk_bidir_fast<IS_RIGHT>(it.ctx.plane.base, (uint32_t)a.g.halo_tpr, tabs, it.wf, it.wb, it.x0, it.y0, a.max_len,
+                                                    left < a.pass_steps ? left : a.pass_steps, &it.st);
             if (r == WALK_CONTINUE && it.st.n < budget_end) {
                 walk_checkpoint(it.st, &ck, &last_f, &last_b);
             } else {
@@ -274,6 +292,8 @@ __device__ __forceinline__ void walk_side(const WalkArgs& a, unsigned int n, uns
 }
 
 __global__ void __launch_bounds__(256) k_walk(const WalkArgs a) {
+    __shared__ __align__(16) uint8_t s_tabs[2 * FID_LUT_SIZE];
+    const StepTabs<uint8_t> tabs = stage_step_tables(a.step_bytes, s_tabs);
     unsigned int nL, nR;
     if (a.round == 0) {
         nL = a.counters->n_starts[0];
@@ -294,8 +314,8 @@ __global__ void __launch_bounds__(256) k_walk(const WalkArgs a) {
     if (nL && wL == 0) wL = 1;
     if (nR && wL >= total_warps) wL = total_warps - 1;
     if (!nR) wL = total_warps;
-    if (nL) walk_side<false>(a, nL, 0, wL);
-    if (nR) walk_side<true>(a, nR, wL, total_warps - wL);
+    if (nL) walk_side<false>(a, tabs, nL, 0, wL);
+    if (nR) walk_side<true>(a, tabs, nR, wL, total_warps - wL);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -303,8 +323,7 @@ __global__ void __launch_bounds__(256) k_walk(const WalkArgs a) {
 // ---------------------------------------------------------------------------------------------------
 struct EmitArgs {
     const uint32_t* halo;
-    const uint32_t* lut_prev;
-    const uint32_t* lut_next;
+    const uint8_t* step_bytes;  // as in WalkArgs
     const SegRec* segs;
     Pt16* points;
     const Counters* counters;
@@ -317,6 +336,8 @@ __global__ void __launch_bounds__(64) k_emit(const EmitArgs a) {
     // One thread per contour segment (contour_walk.cuh): at most ~FID_CKPT_STEP + one walk pass dependent
     // steps each.  Segments are handed out 32 at a time per warp through one atomic, from the END of
     // the list: the long-contour segments of the last walk round start first.
+    __shared__ __align__(16) uint8_t s_tabs[2 * FID_LUT_SIZE];
+    const StepTabs<uint8_t> tabs = stage_step_tables(a.step_bytes, s_tabs);
     unsigned int n = a.counters->n_segs;
     n = n < a.max_segs ? n : a.max_segs;
     const unsigned int lane = threadIdx.x & 31;
@@ -330,8 +351,7 @@ __global__ void __launch_bounds__(64) k_emit(const EmitArgs a) {
             const uint4 w = *reinterpret_cast<const uint4*>(a.segs + (n - 1 - k));
             const SegRec sr{w.x, w.y, w.z, w.w};
             const int f = sr.meta >> 8, s = (sr.meta >> 1) & 0x7F;
-            const WalkCtx ctx{HaloView{a.halo + (size_t)f * a.g.halo_frame_stride + (size_t)s * a.g.halo_scale_stride, a.g.halo_tpr}, a.lut_prev, a.lut_next};
-            trace_segment(ctx, sr, reinterpret_cast<uint32_t*>(a.points));
+            trace_segment(a.halo + (size_t)f * a.g.halo_frame_stride + (size_t)s * a.g.halo_scale_stride, (uint32_t)a.g.halo_tpr, tabs, sr, reinterpret_cast<uint32_t*>(a.points));
         }
         __syncwarp();
     }
