@@ -227,6 +227,7 @@ struct fid_detector {
     std::vector<int32_t> last_conf_counts;
     std::vector<float> last_conf;                    // [last_conf_frames][last_conf_stride]
     bool detected_multi = false;                     // slot 0 holds fid_detect_multi_dict's candidates, not detectMarkers'
+    int inverted = 0;                                // detectInvertedMarker (fid_set_detect_inverted_marker)
     int32_t* d_dbg_rej_n = nullptr;                  // fid_debug_rejected: count, then [max_sel][8] floats
     float* d_dbg_rej = nullptr;
     float stage_ms[ST_COUNT + N_WALK_ROUNDS]{};
@@ -339,10 +340,12 @@ static int configure_kernels(fid_detector* h) {
     CK(cudaFuncSetAttribute(k_threshold<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)thresh_smem_bytes(FID_MAX_WIN_RADIUS)));
     CK(cudaFuncSetAttribute(k_threshold_mma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TM_SMEM_BYTES));
     CK(cudaFuncSetAttribute(k_threshold_mma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TM_SMEM_BYTES));
-    CK(cudaFuncSetAttribute(k_sort_group, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)group_smem(FID_GROUP_MAX_RAW)));
-    for (auto k : {k_identify_retry<false>, k_identify_retry<true>, k_identify_retry<false, true>, k_identify_retry<true, true>})
+    for (auto k : {k_sort_group<false>, k_sort_group<true>}) CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)group_smem(FID_GROUP_MAX_RAW)));
+    for (auto k : {k_identify_retry<false>, k_identify_retry<true>, k_identify_retry<false, true>, k_identify_retry<true, true>, k_identify_retry<false, false, true>,
+                   k_identify_retry<true, false, true>, k_identify_retry<false, true, true>, k_identify_retry<true, true, true>})
         CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kMaxDictMarkers * 4 * 8 + IDENT_WARPS * 256 * 4 + IDENT_WARPS * FID_MAX_WARP_SIDE_SQ)));
-    for (auto k : {k_identify_first<false>, k_identify_first<true>, k_identify_first<false, true>, k_identify_first<true, true>})
+    for (auto k : {k_identify_first<false>, k_identify_first<true>, k_identify_first<false, true>, k_identify_first<true, true>, k_identify_first<false, false, true>,
+                   k_identify_first<true, false, true>, k_identify_first<false, true, true>, k_identify_first<true, true, true>})
         CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kMaxDictMarkers * 4 * 8 + IDENT0_WARPS * 256 * 4 + IDENT0_WARPS * FID_MAX_WARP_SIDE_SQ)));
     return FID_OK;
 }
@@ -903,6 +906,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
     // useAruco3Detection: the stages up to k_finish run on the segmentation plane, a mono8 frame of its own size (gs, seg_src).
     // The threshold-only runs (fid_debug_threshold, fid_debug_time_threshold) stay on the full frame.
     const bool a3 = h->aruco3.enable != 0 && stop_after != ST_THRESH;
+    const bool inv = h->inverted != 0;  // detectInvertedMarker: grouping and identification run their INV instantiations
     A3Geom ag{};
     FrameGeom gs = g;
     const uint8_t* seg_src = d_bgr;
@@ -1109,7 +1113,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.first_list = s.d_first_list;
         static const int group_prof = getenv("FID_GROUP_PROF") ? atoi(getenv("FID_GROUP_PROF")) : 0;
         a.prof = group_prof;
-        launch_prio(k_sort_group, dim3(nf), dim3(GROUP_THREADS), group_smem(h->max_raw), st, 4, a);
+        launch_prio(inv ? k_sort_group<true> : k_sort_group<false>, dim3(nf), dim3(GROUP_THREADS), group_smem(h->max_raw), st, 4, a);
         launches++;
     };
     auto identify = [&](const DevParams& Pd, const unsigned long long* dict) {
@@ -1134,7 +1138,15 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.counters = s.d_counters;
         // fixed grids over work lists: a grid of one block per (frame, candidate slot) is 32 768 blocks of which 1 500 have work
         if (a3) a.pyr = A3Pyramid{s.d_gray, g.gray_frame_stride, s.d_a3_pyr, s.d_raw, ag};
-        if (conf) {  // detectMarkersWithConfidence
+        if (inv) {  // detectInvertedMarker: [useAruco3Detection][detectMarkersWithConfidence]
+            static void (*const first[2][2])(const IdentifyArgs) = {{k_identify_first<false, false, true>, k_identify_first<false, true, true>},
+                                                                    {k_identify_first<true, false, true>, k_identify_first<true, true, true>}};
+            static void (*const retry[2][2])(const IdentifyArgs) = {{k_identify_retry<false, false, true>, k_identify_retry<false, true, true>},
+                                                                    {k_identify_retry<true, false, true>, k_identify_retry<true, true, true>}};
+            if (conf) a.cand_conf = s.d_cand_conf;
+            launch_prio(first[a3][conf], dim3(h->sm_count * 4), dim3(IDENT0_WARPS * 32), ident_smem(Pd, IDENT0_WARPS), st, 4, a);
+            launch_prio(retry[a3][conf], dim3(h->sm_count * 2), dim3(IDENT_WARPS * 32), ident_smem(Pd, IDENT_WARPS), st, 4, a);
+        } else if (conf) {  // detectMarkersWithConfidence
             a.cand_conf = s.d_cand_conf;
             launch_prio(a3 ? k_identify_first<true, true> : k_identify_first<false, true>, dim3(h->sm_count * 4), dim3(IDENT0_WARPS * 32), ident_smem(Pd, IDENT0_WARPS), st, 4, a);
             launch_prio(a3 ? k_identify_retry<true, true> : k_identify_retry<false, true>, dim3(h->sm_count * 2), dim3(IDENT_WARPS * 32), ident_smem(Pd, IDENT_WARPS), st, 4, a);
@@ -1903,6 +1915,16 @@ extern "C" int fid_set_marker_confidence(fid_detector* h, int enable) {
     return FID_OK;
 }
 
+// detectInvertedMarker.  Slot 0's candidates (fid_debug_rejected) came from the other mode once the setting changes.
+extern "C" int fid_set_detect_inverted_marker(fid_detector* h, int enable) {
+    if (!h || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight were enqueued with the old setting
+    if (enable && (h->batch_refine || h->mrefine.enable)) return FID_ERR_UNSUPPORTED;  // refineDetectedMarkers under the flag is not modelled
+    const int v = enable ? 1 : 0;
+    if (v != h->inverted) h->detected = false;
+    h->inverted = v;
+    return FID_OK;
+}
+
 extern "C" int fid_last_marker_confidence(fid_detector* h, int max_markers, int* n_frames, float* out) {
     if (!h || !n_frames || max_markers < 0 || !h->last_conf_valid) return FID_ERR_INVALID_ARG;
     const int nf = h->last_conf_frames;
@@ -2304,6 +2326,7 @@ extern "C" int fid_set_marker_refinement(fid_detector* h, const fid_marker_refin
     if (!h || !params || h->pend_count) return FID_ERR_INVALID_ARG;
     const fid_marker_refine_params p = *params;
     if (p.enable && (!(p.min_rep_distance > 0) || !std::isfinite(p.min_rep_distance) || !std::isfinite(p.error_correction_rate))) return FID_ERR_INVALID_ARG;
+    if (p.enable && h->inverted) return FID_ERR_UNSUPPORTED;  // refineDetectedMarkers with detectInvertedMarker is not modelled
     if (p.enable) {  // (a failed allocation leaves the option off; the next enable completes it)
         CK(cudaSetDevice(h->device));
         int rc;
@@ -2323,6 +2346,7 @@ extern "C" int fid_refine_detected_markers(fid_detector* h, const uint8_t* bgr, 
         (max_markers > 0 && (!ids || !corners)) || n_rejected < 0 || n_rejected > FID_MAX_REJECTED || (n_rejected > 0 && !rejected))
         return FID_ERR_INVALID_ARG;
     if (width < 16 || height < 16 || width > h->max_w || height > h->max_h || stride < (size_t)width * h->bpp) return FID_ERR_INVALID_ARG;
+    if (h->inverted) return FID_ERR_UNSUPPORTED;  // refineDetectedMarkers with detectInvertedMarker is not modelled
     if (!h->mrefine.enable || h->n_boards + h->n_charuco == 0) return FID_ERR_INVALID_ARG;
     if (h->pend_count) return FID_ERR_INVALID_ARG;  // slot 0 may belong to a batch in flight
     CK(cudaSetDevice(h->device));
@@ -2372,7 +2396,7 @@ extern "C" int fid_refine_detected_markers(fid_detector* h, const uint8_t* bgr, 
 
 extern "C" int fid_set_batch_marker_refinement(fid_detector* h, int enable) {
     if (!h || h->pend_count) return FID_ERR_INVALID_ARG;
-    if (enable && (h->multi || h->aruco3.enable || h->marker_conf)) return FID_ERR_UNSUPPORTED;
+    if (enable && (h->multi || h->aruco3.enable || h->marker_conf || h->inverted)) return FID_ERR_UNSUPPORTED;
     if (enable) {  // (a failed allocation leaves the option off; the next enable completes it)
         CK(cudaSetDevice(h->device));
         const size_t F = h->max_batch, M = F * h->max_markers;
@@ -2674,6 +2698,7 @@ extern "C" int fid_debug_rejected(fid_detector* h, int max_rejected, int* n, flo
     if (!h->detected) return FID_ERR_INVALID_ARG;  // slot 0's candidate lists were never written
     if (h->detected_multi) return FID_ERR_UNSUPPORTED;  // detectMarkersMultiDict's rejected list (DESIGN.md finding 15) is not modelled
     if (h->aruco3.enable) return FID_ERR_UNSUPPORTED;   // nor is the rejected list of useAruco3Detection (finding 16)
+    if (h->inverted) return FID_ERR_UNSUPPORTED;        // nor the one of detectInvertedMarker (finding 18)
     CK(cudaSetDevice(h->device));
     int rc;
     if (!h->d_dbg_rej_n && (rc = dalloc(&h->d_dbg_rej_n, 1)) != FID_OK) return rc;

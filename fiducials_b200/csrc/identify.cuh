@@ -149,8 +149,9 @@ FID_HD int otsu_threshold(const int* h, int total) {
 }
 
 struct IdentifyResult {
-    int id;        // -1 = rejected
-    int rotation;  // number of corner rotations to apply
+    int id;         // -1 = rejected
+    int rotation;   // number of corner rotations to apply
+    bool inverted;  // detectInvertedMarker: the cells were read inverted (a white marker on a dark surround)
 };
 
 // The cell bits of a quad (_extractBits): cell c = y*cells + x is bit c of lo for c < 64, bit c-64 of hi otherwise (7x7 markers
@@ -291,11 +292,15 @@ FID_HD float marker_confidence(const int* cnt, const DevParams& P, unsigned long
 // `img` : S*S bytes of scratch, `hist`: 256 ints of scratch (zeroed by this function).
 // dict  : n_markers x 4 rotations packed as little-endian byte strings in 64-bit words.
 // CONF: on a match hist holds the cell counts marker_confidence reads, with word dict[id * 4 + rotation].
-template <bool CONF = false, class Lanes, class Img>
+// INV (detectInvertedMarker, DESIGN.md finding 18 A): the border errors are also counted on the inverted cells, and where they are
+// strictly fewer the candidate continues as a white marker -- the inverted cells go to the border limit and the dictionary search,
+// and under CONF the counts become the inverted window's (win^2 - count), so that the confidence is measured against the polarity
+// that was chosen.  A tie keeps the cells as read.
+template <bool CONF = false, bool INV = false, class Lanes, class Img>
 FID_HD IdentifyResult identify_candidate(const Lanes& L, const Img& gray, int W, int H, const QuadF& quad, const DevParams& P, const unsigned long long* dict, uint8_t* img,
                                          int* hist) {
-    IdentifyResult res = {-1, 0};
-    const CellBits bits = extract_bits<CONF>(L, gray, W, H, quad, P, img, hist);
+    IdentifyResult res = {-1, 0, false};
+    CellBits bits = extract_bits<CONF>(L, gray, W, H, quad, P, img, hist);
     if (!bits.ok) return res;
     // border errors (_getBorderErrors) -- number of white bits in the border ring
     const int cells = P.marker_size + 2 * P.marker_border_bits;
@@ -306,6 +311,21 @@ FID_HD IdentifyResult identify_candidate(const Lanes& L, const Img& gray, int W,
             const bool in_border = y < bb || y >= cells - bb || x < bb || x >= cells - bb;
             if (in_border && bits.at(y * cells + x)) border_errors++;
         }
+    if constexpr (INV) {
+        const int inv_errors = cells * cells - ms * ms - border_errors;  // black bits in the border ring
+        if (inv_errors < border_errors) {
+            border_errors = inv_errors;
+            bits.lo = ~bits.lo;  // bits beyond cells*cells are never read
+            bits.hi = ~bits.hi;
+            res.inverted = true;
+            if constexpr (CONF) {
+                const int margin = (int)(P.ignored_margin_per_cell * P.px_per_cell);
+                const int win = P.px_per_cell - 2 * margin;
+                for (int c = L.lane(); c < cells * cells; c += L.count()) hist[c] = win * win - hist[c];
+                L.sync();
+            }
+        }
+    }
     const int max_border = (int)((double)(ms * ms) * P.max_err_border_rate);
     if (border_errors > max_border) return res;
     const unsigned long long cand = inner_code(bits, P);

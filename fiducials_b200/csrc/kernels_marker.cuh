@@ -104,6 +104,8 @@ struct WarpLanes {
 #define FID_GROUP_MAX_RAW 4096  // >= fid_detector::max_raw
 #define GROUP_CLOSE_SMEM_WORDS 12288  // 48 KB of the close-pair matrix in shared memory
 
+// INV (detectInvertedMarker, DESIGN.md finding 18 B): every group keeps its smallest member (group_finish_lanes<true>).
+template <bool INV = false>
 __global__ void __launch_bounds__(GROUP_THREADS) k_sort_group(const GroupArgs a) {
     const int f = blockIdx.x;
     const int tid = threadIdx.x;
@@ -285,7 +287,7 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_sort_group(const GroupArgs a)
     {
         const WarpLanes L;
         for (int g = tid >> 5; g < s_n_groups; g += GROUP_THREADS / 32)
-            group_finish_lanes(L, g, qs, a.marker_size, a.border_bits, a.min_group_dist, sm_selected, sm_members, &s_members_used, sm_next, sm_head, a.fs.close_count + fo,
+            group_finish_lanes<INV>(L, g, qs, a.marker_size, a.border_bits, a.min_group_dist, sm_selected, sm_members, &s_members_used, sm_next, sm_head, a.fs.close_count + fo,
                                a.fs.close_idx + fo, a.fs.close_off + fo, &s_total_close);
     }
     __syncthreads();
@@ -375,7 +377,9 @@ __device__ __forceinline__ void identify_write(const IdentifyArgs& a, size_t fo,
 // its close contours included, reads the pyramid level its own contour length picks, with the quad scaled to that level.
 // CONF (detectMarkersWithConfidence): each decoded candidate's confidence goes to cand_conf, from the cell counts the attempt
 // that decoded left in its warp's `hist` (identify.cuh, marker_confidence).
-template <bool PYR, bool CONF>
+// INV (detectInvertedMarker): every attempt tries both polarities (identify_candidate<CONF, true>); under CONF the counts left in
+// `hist` are the chosen polarity's.
+template <bool PYR, bool CONF, bool INV>
 __device__ __forceinline__ IdentifyResult identify_attempt(const IdentifyArgs& a, const WarpLanes& L, int f, int level, const QuadF& quad, const unsigned long long* dict,
                                                            uint8_t* img, int* hist) {
     if constexpr (PYR) {
@@ -385,10 +389,10 @@ __device__ __forceinline__ IdentifyResult identify_attempt(const IdentifyArgs& a
             q.x[c] = quad.x[c] * s;
             q.y[c] = quad.y[c] * s;
         }
-        return identify_candidate<CONF>(L, a.pyr.plane(f, level), a.pyr.g.lv[level].W, a.pyr.g.lv[level].H, q, a.P, dict, img, hist);
+        return identify_candidate<CONF, INV>(L, a.pyr.plane(f, level), a.pyr.g.lv[level].W, a.pyr.g.lv[level].H, q, a.P, dict, img, hist);
     } else {
         const FrameImg gray{a.src + (size_t)f * a.frame_stride, a.row_stride, a.enc};
-        return identify_candidate<CONF>(L, gray, a.W, a.H, quad, a.P, dict, img, hist);
+        return identify_candidate<CONF, INV>(L, gray, a.W, a.H, quad, a.P, dict, img, hist);
     }
 }
 template <bool PYR>
@@ -399,7 +403,7 @@ __device__ __forceinline__ int identify_level(const IdentifyArgs& a, size_t fo, 
         return 0;
 }
 
-template <bool PYR, bool CONF = false>
+template <bool PYR, bool CONF = false, bool INV = false>
 __global__ void __launch_bounds__(IDENT0_WARPS * 32) k_identify_first(const IdentifyArgs a) {
     extern __shared__ unsigned long long sm_dict[];  // n_markers*4 words, then per-warp scratch
     const unsigned int n_first = a.counters->n_first;
@@ -416,7 +420,7 @@ __global__ void __launch_bounds__(IDENT0_WARPS * 32) k_identify_first(const Iden
         const int f = (int)(rec >> 16), k = (int)(rec & 0xFFFFu);
         const size_t fo = (size_t)f * a.max_raw, o = (size_t)f * a.max_sel + k;
         const int si = a.fs.sel_idx[fo + k];
-        const IdentifyResult r = identify_attempt<PYR, CONF>(a, L, f, identify_level<PYR>(a, fo, si), a.fs.quads[fo + si], sm_dict, img, hist);
+        const IdentifyResult r = identify_attempt<PYR, CONF, INV>(a, L, f, identify_level<PYR>(a, fo, si), a.fs.quads[fo + si], sm_dict, img, hist);
         __syncwarp();
         if (lane == 0) {
             if (r.id >= 0) {
@@ -436,7 +440,7 @@ __global__ void __launch_bounds__(IDENT0_WARPS * 32) k_identify_first(const Iden
 // One block per candidate whose first attempt failed.  A non-marker group of a dozen nested outlines used to cost a dozen
 // identifications back to back in one warp -- the longest chain of the launch.  Here warp w tries attempts 1 + w, 1 + w + 8, ...
 // concurrently; the lowest successful attempt wins, which is exactly the sequential first-success rule.
-template <bool PYR, bool CONF = false>
+template <bool PYR, bool CONF = false, bool INV = false>
 __global__ void __launch_bounds__(IDENT_WARPS * 32) k_identify_retry(const IdentifyArgs a) {
     extern __shared__ unsigned long long sm_dict[];  // n_markers*4 words, then per-warp scratch
     __shared__ int s_best;                            // lowest successful attempt so far
@@ -463,7 +467,7 @@ __global__ void __launch_bounds__(IDENT_WARPS * 32) k_identify_retry(const Ident
         for (int t = 1 + warp; t <= nc; t += IDENT_WARPS) {
             if (t > *reinterpret_cast<volatile int*>(&s_best)) break;  // an earlier attempt already decoded
             const QuadF quad = a.fs.quads[fo + a.fs.close_idx[fo + co + t - 1]];
-            const IdentifyResult r = identify_attempt<PYR, CONF>(a, L, f, level, quad, sm_dict, img, hist);
+            const IdentifyResult r = identify_attempt<PYR, CONF, INV>(a, L, f, level, quad, sm_dict, img, hist);
             __syncwarp();
             if (r.id >= 0) {
                 if (lane == 0) {

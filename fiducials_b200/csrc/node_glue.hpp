@@ -98,6 +98,9 @@ class FiducialsNode {
         const fid_aruco3_params a{1, min_side, ratio};
         check(fid_set_aruco3(det, &a), "fid_set_aruco3");
     }
+    // White-on-black markers too (new, no reference counterpart): cv2's detectInvertedMarker.  A group of nested outlines then keeps
+    // its smallest, as in cv2, so black markers come back with other corners than without the flag.
+    void setDetectInvertedMarker(bool enable) { check(fid_set_detect_inverted_marker(det, enable ? 1 : 0), "fid_set_detect_inverted_marker"); }
     ~FiducialsNode() {
         if (det) fid_destroy(det);
     }

@@ -201,7 +201,9 @@ FID_HD int group_pairs(int n, const CloseWord& close_word, uint8_t* selected, in
 // count() members against the reference at once and the first hit becomes the new reference, which is the
 // sequential rule.  members: scratch shared by all groups (2 ints per candidate), *members_used /
 // *total_close: reservation counters (atomics on the device).
-template <class Lanes>
+// SMALLEST_FIRST (detectInvertedMarker, DESIGN.md finding 18 B): the members are sorted descending instead -- the group keeps its
+// smallest-perimeter member and collects the close contours from there outward.
+template <bool SMALLEST_FIRST = false, class Lanes>
 FID_HD void group_finish_lanes(const Lanes& L, int g, const QuadF* quads, int marker_size, int border_bits, float min_group_dist, uint8_t* selected, int* members,
                                int* members_used, const int* next_in_group, const int* group_head, int* close_count, int* close_idx, int* close_off, int* total_close) {
     const int lane = L.lane(), width = L.count();
@@ -220,14 +222,14 @@ FID_HD void group_finish_lanes(const Lanes& L, int g, const QuadF* quads, int ma
     if (m <= width) {  // rank sort, one member per lane
         const int mine = lane < m ? mem[lane] : 0x7fffffff;
         int rank = 0;
-        for (int k = 0; k < m; k++) rank += L.shfl_i(mine, k) < mine ? 1 : 0;
+        for (int k = 0; k < m; k++) rank += (SMALLEST_FIRST ? L.shfl_i(mine, k) > mine : L.shfl_i(mine, k) < mine) ? 1 : 0;
         L.sync();
         if (lane < m) mem[rank] = mine;
     } else if (lane == 0) {
         for (int x = 1; x < m; x++) {  // insertion sort (rare: more members than lanes)
             const int v = mem[x];
             int b = x - 1;
-            while (b >= 0 && mem[b] > v) {
+            while (b >= 0 && (SMALLEST_FIRST ? mem[b] < v : mem[b] > v)) {
                 mem[b + 1] = mem[b];
                 b--;
             }
@@ -271,8 +273,8 @@ FID_HD void group_finish_lanes(const Lanes& L, int g, const QuadF* quads, int ma
 // Both passes, serial (CPU harness).  `close_word(i, w)` returns bits [32w, 32w+32) of row i of the pair
 // predicate avgDist(i,j) < perimeter[j] * minMarkerDistanceRate (upper triangle, j > i), `close_word.row_any(i)`
 // whether row i has any bit.  Outputs: selected[i] and, for group leaders, the list of close contours
-// (indices) in close_idx[close_off[i] .. close_off[i] + close_count[i]).
-template <class Lanes, class CloseWord>
+// (indices) in close_idx[close_off[i] .. close_off[i] + close_count[i]).  SMALLEST_FIRST: as group_finish_lanes.
+template <bool SMALLEST_FIRST = false, class Lanes, class CloseWord>
 FID_HD void group_candidates(const Lanes& L, int n, const QuadF* quads, int marker_size, int border_bits, float min_group_dist, const CloseWord& close_word, uint8_t* selected,
                              int* group_id,        // [n]
                              int* group_members,   // [2n]  scratch
@@ -287,7 +289,7 @@ FID_HD void group_candidates(const Lanes& L, int n, const QuadF* quads, int mark
     const int n_groups = group_pairs(n, close_word, selected, group_id, next_in_group, group_head, group_tail, close_count, grouped);
     int total_close = 0, members_used = 0;
     for (int g = 0; g < n_groups; g++)
-        group_finish_lanes(L, g, quads, marker_size, border_bits, min_group_dist, selected, group_members, &members_used, next_in_group, group_head, close_count, close_idx, close_off,
+        group_finish_lanes<SMALLEST_FIRST>(L, g, quads, marker_size, border_bits, min_group_dist, selected, group_members, &members_used, next_in_group, group_head, close_count, close_idx, close_off,
                            &total_close);
 }
 

@@ -209,6 +209,11 @@ class Detector:
         _lib.check(self.lib.fid_last_marker_confidence(self.h, max_markers, C.byref(nf), out.ctypes.data_as(C.c_void_p)), "fid_last_marker_confidence")
         return out
 
+    def set_detect_inverted_marker(self, enable: bool):
+        """fid_set_detect_inverted_marker (detectInvertedMarker): also detect white-on-black markers; a group of nested outlines then
+        keeps its smallest, as in cv2, so black markers can come back with other corners."""
+        _lib.check(self.lib.fid_set_detect_inverted_marker(self.h, int(bool(enable))), "fid_set_detect_inverted_marker")
+
     def set_aruco3(self, min_side: int = 32, ratio: float = 0.0, enable: bool = True):
         """fid_set_aruco3: useAruco3Detection with minSideLengthCanonicalImg = min_side and minMarkerLengthRatioOriginalImg = ratio
         (cv2's defaults 32 and 0); enable=False turns the mode off again."""
@@ -508,7 +513,8 @@ class FiducialsNode:
 
     def __init__(self, dictionary=7, fiducial_len=0.14, ignore_fiducials: Iterable[int] = (), fiducial_len_override: Optional[Dict[int, float]] = None,
                  do_pose_estimation=True, device=0, max_width=1920, max_height=1080, max_batch=1, doCornerRefinement=True, cornerRefinementSubPix=True, pose_hypotheses=False,
-                 boards=(), charuco_boards=(), refine_markers=None, diamonds=None, dictionaries=(), aruco3=None, **detector_params):
+                 boards=(), charuco_boards=(), refine_markers=None, diamonds=None, dictionaries=(), aruco3=None, detect_inverted_marker=False,
+                 **detector_params):
         # doCornerRefinement / cornerRefinementSubPix -> cornerRefinementMethod NONE / SUBPIX / CONTOUR (:700-711, configCallback :274-281)
         if refine_markers is not None and not boards and not charuco_boards:
             raise ValueError("refine_markers needs boards or charuco_boards")
@@ -529,6 +535,10 @@ class FiducialsNode:
         # minSideLengthCanonicalImg) turns on cv2's useAruco3Detection; the messages carry the full-resolution corners it returns
         if aruco3 is not None:
             self.det.set_aruco3(int(aruco3[1]), float(aruco3[0]))
+        # white-on-black markers too (new, no reference counterpart): cv2's detectInvertedMarker; a group of nested outlines then keeps
+        # its smallest, so black markers come back with cv2's corners under the flag, not the reference's
+        if detect_inverted_marker:
+            self.det.set_detect_inverted_marker(True)
         # both planar pose solutions of every marker (new, no reference counterpart): when on, the pose results carry an extra
         # attribute `pose_hypotheses` = {fiducial_id: fid_pose_hypotheses record}; their message fields are unchanged
         self.poseHypotheses = bool(pose_hypotheses)

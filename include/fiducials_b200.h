@@ -425,6 +425,16 @@ int fid_set_marker_confidence(fid_detector* h, int enable);
  * with nothing written, if a frame of the batch has more markers than max_markers. */
 int fid_last_marker_confidence(fid_detector* h, int max_markers, int* n_frames, float* out);
 
+/* detectInvertedMarker of OpenCV 4.13 (default off): also detect white-on-black markers (engraved or laser-etched plates, markers
+ * on dark surfaces, screens).  Every candidate's border is checked in both polarities and read in the one with fewer border errors
+ * (a tie keeps black-on-white); its confidence is measured against that polarity.  As in cv2, the flag also changes which outline
+ * of a group of nested candidates is kept: the smallest instead of the largest, so ordinary black markers come back with other
+ * corners and possibly in another order.  Applies to fid_detect, fid_detect_pose_batch, fid_submit_batch / fid_collect_batch,
+ * fid_detect_multi_dict, fid_detect_with_confidence and useAruco3Detection.  Refused (FID_ERR_UNSUPPORTED, nothing changed), in
+ * both directions: batch marker refinement and marker refinement (fid_set_batch_marker_refinement, fid_set_marker_refinement,
+ * fid_refine_detected_markers); fid_debug_rejected refuses while the flag is on.  Not while batches are in flight. */
+int fid_set_detect_inverted_marker(fid_detector* h, int enable);
+
 /* Pixel format of the frames handed to every entry point that takes `bgr` (default FID_ENC_BGR8).  The
  * reference converts whatever the camera publishes with cv_bridge::toCvCopy(msg, BGR8)
  * (aruco_detect.cpp:348) before detectMarkers turns it into gray again; the library takes the camera's own
