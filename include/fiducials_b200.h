@@ -87,7 +87,15 @@ int fid_set_params(fid_detector* h, const fid_params* params);
  * detectorParams) at aruco_detect.cpp:350.  bgr = H x W x 3 uint8 host pixels (what
  * cv_bridge::toCvCopy(msg, BGR8) yields, :348), `stride` bytes per row.  Outputs (host arrays of
  * capacity max_markers): ids[n], corners[n*8] = x0,y0..x3,y3 in OpenCV's corner order and OpenCV's
- * marker order -- exactly what imageCallback copies into fiducial_msgs/Fiducial (:358-377). */
+ * marker order -- exactly what imageCallback copies into fiducial_msgs/Fiducial (:358-377).
+ * Per-frame capacities (dense calibration targets reach them; DESIGN.md section 3): 4096 raw quad candidates (the quads of every
+ * threshold window before grouping), 512 selected candidates (after grouping) and FID_MAX_MARKERS markers.  Past any of them the call
+ * returns FID_ERR_CAPACITY and still writes *n and ids / corners[0 .. n):
+ *   - more than 256 markers (raw and selected within capacity): n = 256, cv2's first 256 markers in cv2's order, cv2's corners;
+ *   - more than 512 selected: the markers among the first 512 selected candidates (descending perimeter), at most 256;
+ *   - more than 4096 raw candidates: the markers found among 4096 of them, at most 256; which 4096 are kept varies from call to call.
+ *     A frame can get there with fewer than 256 markers (252 markers filling a 3840 x 2160 frame give 4200 raw candidates); fewer
+ *     threshold windows (adaptiveThreshWinSizeMax) reduce the count. */
 int fid_detect(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int max_markers, int* n, int32_t* ids, float* corners);
 
 /* Camera intrinsics as latched by camInfoCallback (aruco_detect.cpp:307-330): K row-major 3x3,
@@ -122,7 +130,11 @@ int fid_pose(fid_detector* h, int n, const int32_t* ids, const float* corners, c
  * bgr + f*frame_stride bytes.  Outputs: counts[f] markers; ids/corners/transforms are dense
  * [n_frames][max_markers] arrays.  `bgr_on_device` != 0 means `bgr` is a device pointer already in
  * HBM (used by bench.py's device-resident figure); otherwise it is (ideally pinned) host memory
- * and the copy is part of the call.  Results always land in host arrays. */
+ * and the copy is part of the call.  Results always land in host arrays.
+ * The per-frame capacities of fid_detect apply to every frame.  The status covers the whole batch: FID_ERR_CAPACITY when any frame
+ * went past one of them (or has more markers than max_markers), and every frame's counts, ids, corners and transforms are written all
+ * the same, each frame as fid_detect describes it; frames within the capacities get exactly the rows they get alone.
+ * fid_collect_batch returns the same status for its batch. */
 int fid_detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, int bgr_on_device, int width, int height, size_t row_stride, size_t frame_stride,
                           const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
                           int max_markers, int32_t* counts, int32_t* ids, float* corners, fid_transform* transforms);
