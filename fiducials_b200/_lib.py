@@ -239,7 +239,7 @@ class fid_map_record(C.Structure):
 # every symbol include/fiducials_b200.h declares (tests/test_abi.py checks the list against the header)
 EXPORTS = [
     "fid_strerror", "fid_version", "fid_default_params", "fid_create", "fid_destroy", "fid_set_params", "fid_detect", "fid_pose",
-    "fid_detect_pose_batch", "fid_submit_batch", "fid_collect_batch", "fid_set_pose_hypotheses", "fid_pose_hypotheses", "fid_last_pose_hypotheses", "fid_set_boards", "fid_estimate_board_poses", "fid_last_board_poses", "fid_set_charuco_boards", "fid_detect_charuco", "fid_last_charuco", "fid_set_marker_refinement", "fid_refine_detected_markers", "fid_set_batch_marker_refinement", "fid_last_marker_refinement", "fid_set_diamonds", "fid_detect_diamonds", "fid_last_diamonds", "fid_set_dictionaries", "fid_detect_multi_dict", "fid_last_dict_indices", "fid_set_aruco3", "fid_debug_aruco3_planes", "fid_detect_with_confidence", "fid_set_marker_confidence", "fid_last_marker_confidence", "fid_set_detect_inverted_marker", "fid_hint_next", "fid_set_input_encoding", "fid_timer_start", "fid_timer_stop", "fid_host_alloc", "fid_host_free", "fid_device_alloc", "fid_device_free", "fid_memcpy_h2d", "fid_debug_threshold", "fid_debug_time_threshold",
+    "fid_detect_pose_batch", "fid_submit_batch", "fid_collect_batch", "fid_set_pose_hypotheses", "fid_pose_hypotheses", "fid_last_pose_hypotheses", "fid_set_boards", "fid_estimate_board_poses", "fid_last_board_poses", "fid_set_charuco_boards", "fid_detect_charuco", "fid_last_charuco", "fid_set_marker_refinement", "fid_refine_detected_markers", "fid_set_batch_marker_refinement", "fid_last_marker_refinement", "fid_set_diamonds", "fid_detect_diamonds", "fid_last_diamonds", "fid_set_dictionaries", "fid_set_family_boards", "fid_set_family_charuco_boards", "fid_set_family_diamonds", "fid_detect_multi_dict", "fid_last_dict_indices", "fid_set_aruco3", "fid_debug_aruco3_planes", "fid_detect_with_confidence", "fid_set_marker_confidence", "fid_last_marker_confidence", "fid_set_detect_inverted_marker", "fid_hint_next", "fid_set_input_encoding", "fid_timer_start", "fid_timer_stop", "fid_host_alloc", "fid_host_free", "fid_device_alloc", "fid_device_free", "fid_memcpy_h2d", "fid_debug_threshold", "fid_debug_time_threshold",
     "fid_debug_candidates", "fid_debug_rejected", "fid_last_stage_ms", "fid_last_counters", "fid_map_default_params", "fid_map_create", "fid_map_destroy", "fid_map_clear",
     "fid_map_load", "fid_map_links", "fid_map_add_links", "fid_map_update", "fid_map_update_sequence", "fid_map_update_frames", "fid_map_update_frames_async", "fid_map_sync", "fid_map_entries", "fid_map_export", "fid_map_merge", "fid_map_export_device",
     "fid_map_merge_device", "fid_map_merge_device_async", "fid_map_export_async", "fid_map_stream", "fid_map_merged_entries", "fid_map_adopt_merged", "fid_map_add_fiducial", "fid_map_refine_default_params", "fid_map_refine",
@@ -287,6 +287,9 @@ def load():
     lib.fid_detect_diamonds.argtypes = [vp, vp, i32, i32, sz, i32, vp, vp, C.POINTER(fid_camera), C.POINTER(i32), vp]
     lib.fid_last_diamonds.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
     lib.fid_set_dictionaries.argtypes = [vp, i32, vp]
+    lib.fid_set_family_boards.argtypes = [vp, i32, vp, vp]
+    lib.fid_set_family_charuco_boards.argtypes = [vp, i32, vp, vp]
+    lib.fid_set_family_diamonds.argtypes = [vp, C.POINTER(fid_diamond_params), C.c_int32]
     lib.fid_detect_multi_dict.argtypes = [vp, vp, i32, i32, sz, i32, C.POINTER(i32), vp, vp, vp]
     lib.fid_last_dict_indices.argtypes = [vp, i32, C.POINTER(i32), vp]
     lib.fid_set_aruco3.argtypes = [vp, C.POINTER(fid_aruco3_params)]

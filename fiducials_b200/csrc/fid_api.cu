@@ -76,6 +76,7 @@ struct Slot {
     int32_t* d_md_ids = nullptr;                       // [n_dicts][max_batch][max_markers]
     float* d_md_corners = nullptr;                     // [n_dicts][max_batch][max_markers][8]
     int32_t* d_out_dict = nullptr;                     // [max_batch][max_markers]          k_dict_merge
+    int32_t* d_md_run = nullptr;                       // [max_batch][FID_MAX_DICTIONARIES + 1] k_dict_merge: each dictionary's run
     // fid_set_aruco3: allocated by the first enable (level 0 of the pyramid is d_gray)
     uint8_t* d_a3_pyr = nullptr;                       // [max_batch][levels 1.. of the largest frame]
     uint8_t* d_a3_seg = nullptr;                       // [max_batch][the largest segmentation plane of the mode's parameters]
@@ -170,6 +171,8 @@ struct fid_detector {
     std::vector<struct fid_pose_hypotheses> last_hyp;  // [last_hyp_frames][last_hyp_stride]
     // one pose per board (fid_set_boards / fid_estimate_board_poses / fid_last_board_poses)
     int n_boards = 0;                                // 0 = off
+    bool board_bound = false;                        // set with fid_set_family_boards: board_fam holds each board's dictionary index
+    int32_t board_fam[FID_MAX_BOARDS]{};
     int32_t *d_board_off = nullptr, *d_board_keys = nullptr, *d_board_marker = nullptr;  // see BoardPoseArgs
     float* d_board_obj = nullptr;
     int32_t* d_board_count = nullptr;                // fid_estimate_board_poses: the list's length
@@ -179,6 +182,9 @@ struct fid_detector {
     std::vector<fid_board_pose> last_board;          // [last_board_frames][last_board_n]
     // ChArUco boards (fid_set_charuco_boards / fid_detect_charuco / fid_last_charuco)
     int n_charuco = 0, charuco_slots = 0;            // 0 = off; slots = corners of all boards
+    bool charuco_bound = false;                      // set with fid_set_family_charuco_boards
+    int32_t charuco_fam[FID_MAX_CHARUCO_BOARDS]{};
+    int32_t charuco_nm[FID_MAX_CHARUCO_BOARDS]{};    // each board's marker count (fid_set_dictionaries checks it against the family)
     CharucoBoardDev* d_ch_boards = nullptr;
     int32_t *d_ch_keys = nullptr, *d_ch_marker = nullptr, *d_ch_ids = nullptr, *d_ch_near_n = nullptr, *d_ch_near_idx = nullptr, *d_ch_near_corner = nullptr;
     float *d_ch_obj = nullptr, *d_ch_chess = nullptr, *d_ch_masks = nullptr;
@@ -203,6 +209,8 @@ struct fid_detector {
     std::vector<float> last_mr_rej;                   // frame after frame, last_mr_nrej[f] x 8 each
     // ChArUco diamonds (fid_set_diamonds / fid_detect_diamonds / fid_last_diamonds)
     fid_diamond_params diamond{};                    // enable = 0: off
+    bool diamond_bound = false;                      // set with fid_set_family_diamonds
+    int32_t diamond_fam = 0;
     DiamondLayout diamond_layout{};
     int32_t* d_dia_io = nullptr;                     // fid_detect_diamonds: the list's length, the diamonds found
     fid_diamond* d_dia_list = nullptr;               // fid_detect_diamonds output, FID_MAX_DIAMONDS records
@@ -421,7 +429,7 @@ static void free_slot(Slot& s) {
                      s.fs.sel_idx,    s.d_nsel,          s.d_nrawc,         s.d_cand_id,      s.d_cand_corners, s.d_out_count,    s.d_out_ids,     s.d_out_corners,
                      s.d_out_tf,      s.fs.raw_of_sorted, s.d_cand_raw,     s.d_first_list,   s.d_retry_list, s.d_out_hyp, s.d_out_board, s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy,
                      s.d_rej_n,       s.d_rej,           s.d_mr_nrec,       s.d_mr_idx,       s.d_mr_board,    s.d_dia_n,       s.d_dia,
-                     s.d_md_count,    s.d_md_ids,        s.d_md_corners,    s.d_out_dict,     s.d_a3_pyr,      s.d_a3_seg,      s.d_cand_conf,   s.d_out_conf};
+                     s.d_md_count,    s.d_md_ids,        s.d_md_corners,    s.d_out_dict,     s.d_md_run,      s.d_a3_pyr,      s.d_a3_seg,      s.d_cand_conf,   s.d_out_conf};
     for (void* p : dptrs)
         if (p) cudaFree(p);
     void* hptrs[] = {s.h_out_count, s.h_out_ids, s.h_out_corners, s.h_out_tf, s.h_counters, s.h_nsel, s.h_nrawc, s.h_out_hyp, s.h_out_board, s.h_out_ch, s.h_out_ch_ids, s.h_out_ch_xy,
@@ -656,7 +664,16 @@ extern "C" int fid_set_dictionaries(fid_detector* h, int n, const fid_dictionary
         if ((int64_t)specs[d].id_offset + dp[d].n_markers - 1 > INT32_MAX) return FID_ERR_INVALID_ARG;  // a published id would overflow
     }
     const bool multi = n > 1 || specs[0].id_offset != 0 || specs[0].fiducial_len > 0;
-    if (multi && (h->n_boards || h->n_charuco || h->batch_refine || h->diamond.enable || h->aruco3.enable || h->marker_conf)) return FID_ERR_UNSUPPORTED;
+    // a board set without a family is ambiguous with several dictionaries
+    if (multi && ((h->n_boards && !h->board_bound) || (h->n_charuco && !h->charuco_bound) || (h->diamond.enable && !h->diamond_bound) || h->batch_refine ||
+                  h->aruco3.enable || h->marker_conf))
+        return FID_ERR_UNSUPPORTED;
+    // every bound family must still exist, and a ChArUco board must fit its family's dictionary
+    for (int b = 0; b < h->n_boards; b++)
+        if (h->board_bound && h->board_fam[b] >= n) return FID_ERR_INVALID_ARG;
+    for (int b = 0; b < h->n_charuco; b++)
+        if (h->charuco_bound && (h->charuco_fam[b] >= n || h->charuco_nm[b] > dp[h->charuco_fam[b]].n_markers)) return FID_ERR_INVALID_ARG;
+    if (h->diamond.enable && h->diamond_bound && h->diamond_fam >= n) return FID_ERR_INVALID_ARG;
     CK(cudaSetDevice(h->device));
     if (multi) {  // (a failed allocation leaves the handle as it was; the next call completes it)
         const size_t F = h->max_batch, M = F * h->max_markers, ND = FID_MAX_DICTIONARIES;
@@ -667,6 +684,7 @@ extern "C" int fid_set_dictionaries(fid_detector* h, int n, const fid_dictionary
             if (!s.d_md_ids && (rc = dalloc(&s.d_md_ids, ND * M)) != FID_OK) return rc;
             if (!s.d_md_corners && (rc = dalloc(&s.d_md_corners, ND * M * 8)) != FID_OK) return rc;
             if (!s.d_out_dict && (rc = dalloc(&s.d_out_dict, M)) != FID_OK) return rc;
+            if (!s.d_md_run && (rc = dalloc(&s.d_md_run, F * (ND + 1))) != FID_OK) return rc;
             if (!s.h_out_dict && (rc = halloc(&s.h_out_dict, M)) != FID_OK) return rc;
         }
     }
@@ -740,6 +758,7 @@ static BoardPoseArgs board_args(const fid_detector* h, const int32_t* count, con
     a.board_keys = h->d_board_keys;
     a.board_marker = h->d_board_marker;
     a.board_obj = h->d_board_obj;
+    for (int b = 0; b < h->n_boards; b++) a.family[b] = h->board_fam[b];
     a.cam = make_camera(cam);
     a.out = out;
     return a;
@@ -821,7 +840,9 @@ static DiamondArgs diamond_args(const fid_detector* h, const uint8_t* src, size_
     a.enc = h->enc;
     a.W = W;
     a.H = H;
-    a.P = h->P;
+    a.P = h->dict_P[h->diamond_fam];  // the cornerSubPix of the markers the loop takes reads the family's parameters
+    a.family = h->diamond_fam;
+    a.id_offset = h->dict_spec[h->diamond_fam].id_offset;
     a.subpix_masks = h->d_subpix_masks;
     a.ch_masks = h->d_ch_masks;
     a.layout = h->diamond_layout;
@@ -1216,6 +1237,35 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
             launches++;
         }
     };
+    // The opt-in board stages over the frame's final markers.  run = nullptr: every marker; in multi-dictionary mode k_dict_merge's
+    // per-frame runs, so that each board, ChArUco board and the diamonds read their family's markers alone.
+    auto board_stages = [&](const int32_t* run) {
+        if (h->n_boards && cam) {  // one pose per (frame, board) (fid_set_boards / fid_set_family_boards)
+            BoardPoseArgs a = board_args(h, s.d_out_count, s.d_out_ids, s.d_out_corners, h->max_markers, cam, s.d_out_board);
+            a.run = run;
+            launch_prio(k_board_pose, dim3(nf * h->n_boards), dim3(FID_BOARD_LANES), 0, st, 5, a);
+            launches++;
+        }
+        if (h->n_charuco) {  // ChArUco corners (and pose with a camera) per (frame, board) (fid_set_charuco_boards / fid_set_family_charuco_boards)
+            CharucoArgs a = charuco_args(h, d_bgr, g.bgr_row_stride, g.bgr_frame_stride, g.W, g.H, s.d_out_count, s.d_out_ids, s.d_out_corners, h->max_markers, cam,
+                                         s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy);
+            a.run = run;
+            launch_prio(k_charuco, dim3(nf * h->n_charuco), dim3(CHARUCO_THREADS), CHARUCO_SMEM, st, 5, a);
+            launches++;
+        }
+        if (diamonds) {  // ChArUco diamonds per frame, from the final markers (fid_set_diamonds / fid_set_family_diamonds)
+            DiamondArgs a = diamond_args(h, d_bgr, g.bgr_row_stride, g.bgr_frame_stride, g.W, g.H, cam);
+            a.max_markers = h->max_markers;
+            a.count = s.d_out_count;
+            a.ids = s.d_out_ids;
+            a.corners = s.d_out_corners;
+            a.run = run;
+            a.n_out = s.d_dia_n;
+            a.out = s.d_dia;
+            launch_prio(k_diamond, dim3(nf), dim3(DIAMOND_THREADS), 0, st, 5, a);
+            launches++;
+        }
+    };
     if (multi) {  // several dictionaries (fid_set_dictionaries): the front end above ran once
         const size_t F = h->max_batch, dstride = F * h->max_markers;
         int grouped = -1;
@@ -1255,11 +1305,13 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.out_ids = s.d_out_ids;
         a.out_corners = s.d_out_corners;
         a.out_dict = s.d_out_dict;
+        a.out_run = s.d_md_run;
         a.out_tf = s.d_out_tf;
         a.out_hyp = (h->pose_hyp && cam) ? s.d_out_hyp : nullptr;
         a.counters = s.d_counters;
         launch_prio(k_dict_merge, dim3(nf), dim3(DICT_MERGE_THREADS), 0, st, 5, a);
         launches++;
+        board_stages(s.d_md_run);
         CK(cudaEventRecord(s.ev[ST_D2H], st));
         h->counters[6] += launches;
         CK(cudaGetLastError());
@@ -1360,28 +1412,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         launch_prio(k_pose_hypotheses, dim3(nf), dim3(POSE_HYP_THREADS), 0, st, 5, a);
         launches++;
     }
-    if (h->n_boards && cam) {  // opt-in: one pose per (frame, board) over the markers k_finish wrote (fid_set_boards)
-        launch_prio(k_board_pose, dim3(nf * h->n_boards), dim3(FID_BOARD_LANES), 0, st, 5,
-                    board_args(h, s.d_out_count, s.d_out_ids, s.d_out_corners, h->max_markers, cam, s.d_out_board));
-        launches++;
-    }
-    if (h->n_charuco) {  // opt-in: ChArUco corners (and pose with a camera) per (frame, board) (fid_set_charuco_boards)
-        launch_prio(k_charuco, dim3(nf * h->n_charuco), dim3(CHARUCO_THREADS), CHARUCO_SMEM, st, 5,
-                    charuco_args(h, d_bgr, g.bgr_row_stride, g.bgr_frame_stride, g.W, g.H, s.d_out_count, s.d_out_ids, s.d_out_corners, h->max_markers, cam,
-                                 s.d_out_ch, s.d_out_ch_ids, s.d_out_ch_xy));
-        launches++;
-    }
-    if (diamonds) {  // opt-in: ChArUco diamonds per frame, from the final markers (fid_set_diamonds)
-        DiamondArgs a = diamond_args(h, d_bgr, g.bgr_row_stride, g.bgr_frame_stride, g.W, g.H, cam);
-        a.max_markers = h->max_markers;
-        a.count = s.d_out_count;
-        a.ids = s.d_out_ids;
-        a.corners = s.d_out_corners;
-        a.n_out = s.d_dia_n;
-        a.out = s.d_dia;
-        launch_prio(k_diamond, dim3(nf), dim3(DIAMOND_THREADS), 0, st, 5, a);
-        launches++;
-    }
+    if (!h->multi) board_stages(nullptr);  // (fid_detect on a multi-dictionary handle is detectMarkers with dictionary 0: no board stage)
     CK(cudaEventRecord(s.ev[ST_D2H], st));
     h->counters[6] += launches;
     CK(cudaGetLastError());
@@ -1629,7 +1660,7 @@ static int detect_pose_batch(fid_detector* h, int n_frames, const uint8_t* bgr, 
     struct fid_pose_hypotheses* hyps = begin_last_hypotheses(h, hyp, n_frames, max_markers);
     const bool brd = h->n_boards && cam;
     fid_board_pose* boards = begin_last_boards(h, brd, n_frames);
-    const bool chr = h->n_charuco > 0;
+    const bool chr = h->n_charuco > 0 && multi == h->multi;  // (not fid_detect on a multi-dictionary handle: enqueue_pipeline)
     begin_last_charuco(h, chr, n_frames);
     const bool mr = may_refine && batch_refines(h);
     begin_last_refinement(h, mr, n_frames);
@@ -2101,10 +2132,20 @@ extern "C" int fid_last_pose_hypotheses(fid_detector* h, int max_markers, int* n
     return FID_OK;
 }
 
-extern "C" int fid_set_boards(fid_detector* h, int n_boards, const fid_board* boards) {
+// Validates a family list (fid_set_family_*): every index must name an entry of the handle's dictionary list.
+static bool families_valid(const fid_detector* h, int n, const int32_t* family) {
+    if (n > 0 && !family) return false;
+    for (int i = 0; i < n; i++)
+        if (family[i] < 0 || family[i] >= h->n_dicts) return false;
+    return true;
+}
+
+// fid_set_boards (family = nullptr: no family, refused in multi-dictionary mode) and fid_set_family_boards
+static int set_boards(fid_detector* h, int n_boards, const fid_board* boards, const int32_t* family) {
     if (!h || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight read the board tables
     if (n_boards < 0 || n_boards > FID_MAX_BOARDS || (n_boards > 0 && !boards)) return FID_ERR_INVALID_ARG;
-    if (n_boards > 0 && h->multi) return FID_ERR_UNSUPPORTED;  // which family a board's ids belong to is not modelled
+    if (family && !families_valid(h, n_boards, family)) return FID_ERR_INVALID_ARG;
+    if (n_boards > 0 && h->multi && !family) return FID_ERR_UNSUPPORTED;  // a board without a family is ambiguous with several dictionaries
     std::vector<int32_t> off(1, 0), keys, marker;
     std::vector<float> obj;
     for (int b = 0; b < n_boards; b++) {
@@ -2146,12 +2187,22 @@ extern "C" int fid_set_boards(fid_detector* h, int n_boards, const fid_board* bo
     CK(cudaMemcpy(h->d_board_keys, keys.data(), sizeof(int32_t) * keys.size(), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(h->d_board_marker, marker.data(), sizeof(int32_t) * marker.size(), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(h->d_board_obj, obj.data(), sizeof(float) * obj.size(), cudaMemcpyHostToDevice));
+    for (int b = 0; b < n_boards; b++) h->board_fam[b] = family ? family[b] : 0;
+    h->board_bound = family != nullptr;
     h->n_boards = n_boards;
     return FID_OK;
 }
 
+extern "C" int fid_set_boards(fid_detector* h, int n_boards, const fid_board* boards) { return set_boards(h, n_boards, boards, nullptr); }
+
+extern "C" int fid_set_family_boards(fid_detector* h, int n_boards, const fid_board* boards, const int32_t* dict_index) {
+    if (!dict_index) return FID_ERR_INVALID_ARG;
+    return set_boards(h, n_boards, boards, dict_index);
+}
+
 extern "C" int fid_estimate_board_poses(fid_detector* h, int n, const int32_t* ids, const float* corners, const fid_camera* cam, fid_board_pose* out) {
     if (!h || n < 0 || n > FID_MAX_MARKERS || !cam || !out || (n > 0 && (!ids || !corners)) || h->n_boards == 0) return FID_ERR_INVALID_ARG;
+    if (h->multi) return FID_ERR_UNSUPPORTED;  // the list carries no family: the batch calls serve this mode
     CK(cudaSetDevice(h->device));
     if (n > 0) {
         CK(cudaMemcpyAsync(h->d_pose_ids, ids, sizeof(int32_t) * n, cudaMemcpyHostToDevice, h->stream));
@@ -2176,10 +2227,12 @@ extern "C" int fid_last_board_poses(fid_detector* h, int max_boards, int* n_fram
     return FID_OK;
 }
 
-extern "C" int fid_set_charuco_boards(fid_detector* h, int n_boards, const fid_charuco_board* boards) {
+// fid_set_charuco_boards (family = nullptr) and fid_set_family_charuco_boards, as set_boards
+static int set_charuco_boards(fid_detector* h, int n_boards, const fid_charuco_board* boards, const int32_t* family) {
     if (!h || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight read the board tables
     if (n_boards < 0 || n_boards > FID_MAX_CHARUCO_BOARDS || (n_boards > 0 && !boards)) return FID_ERR_INVALID_ARG;
-    if (n_boards > 0 && h->multi) return FID_ERR_UNSUPPORTED;
+    if (family && !families_valid(h, n_boards, family)) return FID_ERR_INVALID_ARG;
+    if (n_boards > 0 && h->multi && !family) return FID_ERR_UNSUPPORTED;
     std::vector<CharucoBoardDev> bd;
     std::vector<int32_t> keys, marker, ids, near_n, near_idx, near_corner;
     std::vector<float> obj, chess;
@@ -2190,8 +2243,8 @@ extern "C" int fid_set_charuco_boards(fid_detector* h, int n_boards, const fid_c
         if (!(C.square_length > 0) || !(C.marker_length > 0) || !(C.marker_length < C.square_length) || !std::isfinite(C.square_length)) return FID_ERR_INVALID_ARG;
         if (C.min_markers < 0 || C.min_markers > 2) return FID_ERR_INVALID_ARG;  // cv2 asserts outside 0..2
         const int nm = charuco_n_markers(sx, sy), nc = charuco_n_corners(sx, sy);
-        if (nm > h->P.n_markers) return FID_ERR_INVALID_ARG;  // more markers than the dictionary has
-        CharucoBoardDev d{nm, nc, (int)ids.size(), (int)near_n.size(), C.min_markers, C.check_markers ? 1 : 0};
+        if (nm > h->dict_P[family ? family[b] : 0].n_markers) return FID_ERR_INVALID_ARG;  // more markers than the dictionary has
+        CharucoBoardDev d{nm, nc, (int)ids.size(), (int)near_n.size(), C.min_markers, C.check_markers ? 1 : 0, family ? family[b] : 0};
         std::vector<int32_t> bid(nm);
         for (int i = 0; i < nm; i++) bid[i] = C.ids ? C.ids[i] : i;
         std::vector<int32_t> ord(nm);
@@ -2275,14 +2328,27 @@ extern "C" int fid_set_charuco_boards(fid_detector* h, int n_boards, const fid_c
     CK(cudaMemcpy(h->d_ch_near_corner, near_corner.data(), sizeof(int32_t) * near_corner.size(), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(h->d_ch_obj, obj.data(), sizeof(float) * obj.size(), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(h->d_ch_chess, chess.data(), sizeof(float) * chess.size(), cudaMemcpyHostToDevice));
+    for (int b = 0; b < n_boards; b++) {
+        h->charuco_fam[b] = family ? family[b] : 0;
+        h->charuco_nm[b] = bd[b].n_markers;
+    }
+    h->charuco_bound = family != nullptr;
     h->n_charuco = n_boards;
     h->charuco_slots = slots;
     return FID_OK;
 }
 
+extern "C" int fid_set_charuco_boards(fid_detector* h, int n_boards, const fid_charuco_board* boards) { return set_charuco_boards(h, n_boards, boards, nullptr); }
+
+extern "C" int fid_set_family_charuco_boards(fid_detector* h, int n_boards, const fid_charuco_board* boards, const int32_t* dict_index) {
+    if (!dict_index) return FID_ERR_INVALID_ARG;
+    return set_charuco_boards(h, n_boards, boards, dict_index);
+}
+
 extern "C" int fid_detect_charuco(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int n, const int32_t* ids, const float* corners,
                                   const fid_camera* cam, fid_charuco_result* results, int32_t* corner_ids, float* corner_xy) {
     if (!h || !bgr || n < 0 || n > FID_MAX_MARKERS || (n > 0 && (!ids || !corners)) || !results || !corner_ids || !corner_xy || h->n_charuco == 0) return FID_ERR_INVALID_ARG;
+    if (h->multi) return FID_ERR_UNSUPPORTED;  // the list carries no family: the batch calls serve this mode
     if (width < 16 || height < 16 || width > h->max_w || height > h->max_h || stride < (size_t)width * h->bpp) return FID_ERR_INVALID_ARG;
     if (h->pend_count) return FID_ERR_INVALID_ARG;  // slot 0 may belong to a batch in flight
     CK(cudaSetDevice(h->device));
@@ -2348,6 +2414,7 @@ extern "C" int fid_refine_detected_markers(fid_detector* h, const uint8_t* bgr, 
     if (width < 16 || height < 16 || width > h->max_w || height > h->max_h || stride < (size_t)width * h->bpp) return FID_ERR_INVALID_ARG;
     if (h->inverted) return FID_ERR_UNSUPPORTED;  // refineDetectedMarkers with detectInvertedMarker is not modelled
     if (!h->mrefine.enable || h->n_boards + h->n_charuco == 0) return FID_ERR_INVALID_ARG;
+    if (h->multi) return FID_ERR_UNSUPPORTED;  // the lists carry no family
     if (h->pend_count) return FID_ERR_INVALID_ARG;  // slot 0 may belong to a batch in flight
     CK(cudaSetDevice(h->device));
     Slot& s = h->slot[0];
@@ -2445,10 +2512,12 @@ extern "C" int fid_last_marker_refinement(fid_detector* h, int max_markers, int 
     return FID_OK;
 }
 
-extern "C" int fid_set_diamonds(fid_detector* h, const fid_diamond_params* params) {
+// fid_set_diamonds (family < 0: no family, refused in multi-dictionary mode) and fid_set_family_diamonds
+static int set_diamonds(fid_detector* h, const fid_diamond_params* params, int32_t family) {
     if (!h || !params || h->pend_count) return FID_ERR_INVALID_ARG;  // batches in flight read the layout
     const fid_diamond_params p = *params;
-    if (p.enable && h->multi) return FID_ERR_UNSUPPORTED;
+    if (family >= h->n_dicts) return FID_ERR_INVALID_ARG;
+    if (p.enable && h->multi && family < 0) return FID_ERR_UNSUPPORTED;
     DiamondLayout L{};
     if (p.enable) {
         if (!std::isfinite(p.square_length) || !(p.marker_length > 0) || !(p.marker_length < p.square_length)) return FID_ERR_INVALID_ARG;
@@ -2476,12 +2545,22 @@ extern "C" int fid_set_diamonds(fid_detector* h, const fid_diamond_params* param
     h->diamond = p;
     h->diamond.enable = p.enable ? 1 : 0;
     h->diamond_layout = L;
+    h->diamond_fam = family < 0 ? 0 : family;
+    h->diamond_bound = family >= 0;
     return FID_OK;
+}
+
+extern "C" int fid_set_diamonds(fid_detector* h, const fid_diamond_params* params) { return set_diamonds(h, params, -1); }
+
+extern "C" int fid_set_family_diamonds(fid_detector* h, const fid_diamond_params* params, int32_t dict_index) {
+    if (dict_index < 0) return FID_ERR_INVALID_ARG;
+    return set_diamonds(h, params, dict_index);
 }
 
 extern "C" int fid_detect_diamonds(fid_detector* h, const uint8_t* bgr, int width, int height, size_t stride, int n, const int32_t* ids, const float* corners,
                                    const fid_camera* cam, int* n_diamonds, fid_diamond* out) {
     if (!h || !bgr || !n_diamonds || n < 0 || n > FID_MAX_MARKERS || (n > 0 && (!ids || !corners)) || (n >= 4 && !out) || !h->diamond.enable) return FID_ERR_INVALID_ARG;
+    if (h->multi) return FID_ERR_UNSUPPORTED;  // the list carries no family: the batch calls serve this mode
     if (width < 16 || height < 16 || width > h->max_w || height > h->max_h || stride < (size_t)width * h->bpp) return FID_ERR_INVALID_ARG;
     if (h->pend_count) return FID_ERR_INVALID_ARG;  // slot 0 may belong to a batch in flight
     CK(cudaSetDevice(h->device));

@@ -1019,9 +1019,20 @@ struct BoardPoseArgs {
     const int32_t* board_keys;    //                       its ids, sorted
     const int32_t* board_marker;  //                       the marker (row within the board) of each sorted id
     const float* board_obj;       // [rows][4][3]          object points, in the board's own marker order
+    const int32_t* run;           // [F][FID_MAX_DICTIONARIES + 1] family runs of the merged list (k_dict_merge), or nullptr: every marker
+    int32_t family[FID_MAX_BOARDS];  //                    each board's dictionary index (read with run only)
     Camera cam;
     fid_board_pose* out;          // [F][n_boards]
 };
+
+// Multi-dictionary mode: a family's markers are one contiguous run of the frame's merged list (DESIGN.md finding 19), so a stage
+// bound to family k reads that run as the frame's list: corners[di == k], ids[di == k] in list order.
+__device__ __forceinline__ void family_run(const int32_t* run, int f, int family, const int32_t** ids, const float** corners, int* n) {
+    const int32_t* r = run + (size_t)f * (FID_MAX_DICTIONARIES + 1) + family;
+    *ids += r[0];
+    *corners += (size_t)r[0] * 8;
+    *n = r[1] - r[0];
+}
 
 #define BOARD_POSE_MAX_POINTS (4 * FID_MAX_MARKERS)
 
@@ -1033,10 +1044,11 @@ __global__ void __launch_bounds__(FID_BOARD_LANES) k_board_pose(const BoardPoseA
     __shared__ double s_mn[BOARD_POSE_MAX_POINTS * 2];
     const int f = blockIdx.x / a.n_boards, b = blockIdx.x % a.n_boards;
     const int lane = threadIdx.x;
-    const int n = min(a.count[f], FID_MAX_MARKERS);
+    int n = min(a.count[f], FID_MAX_MARKERS);
     const int off = a.board_off[b], nb = a.board_off[b + 1] - off;
     const int32_t* ids = a.ids + (size_t)f * a.max_markers;
     const float* corners = a.corners + (size_t)f * a.max_markers * 8;
+    if (a.run) family_run(a.run, f, a.family[b], &ids, &corners, &n);
     int m = 0;
     for (int j0 = 0; j0 < n; j0 += FID_BOARD_LANES) {
         const int j = j0 + lane;
@@ -1075,6 +1087,7 @@ struct CharucoBoardDev {
     int n_markers, n_corners;
     int marker_off, corner_off;  // rows of the marker tables / of the corner tables; corner_off is also the board's first output slot
     int min_markers, check_markers;
+    int family;                  // its dictionary index (read with CharucoArgs::run only)
 };
 
 struct CharucoArgs {
@@ -1092,6 +1105,7 @@ struct CharucoArgs {
     const float* chess;                           // corner tables
     const int32_t *near_n, *near_idx, *near_corner;
     const float* masks;      // charuco_subpix_masks
+    const int32_t* run;      // as BoardPoseArgs; each board's family is CharucoBoardDev::family
     int win_default, max_iters;
     double eps_sq;
     int has_cam;
@@ -1138,9 +1152,10 @@ __global__ void __launch_bounds__(CHARUCO_THREADS) k_charuco(const CharucoArgs a
     const CharucoView B{bd.n_markers, bd.n_corners, bd.min_markers, bd.check_markers, a.keys + bd.marker_off, a.marker_of + bd.marker_off, a.board_ids + bd.marker_off,
                         a.obj + (size_t)bd.marker_off * 12, a.chess + (size_t)bd.corner_off * 3, a.near_n + bd.corner_off, a.near_idx + 2 * bd.corner_off,
                         a.near_corner + 2 * bd.corner_off};
-    const int n = min(a.count[f], FID_MAX_MARKERS);
+    int n = min(a.count[f], FID_MAX_MARKERS);
     const int32_t* ids = a.ids + (size_t)f * a.max_markers;
     const float* corners = a.corners + (size_t)f * a.max_markers * 8;
+    if (a.run) family_run(a.run, f, bd.family, &ids, &corners, &n);
     for (int j = tid; j < n; j += CHARUCO_THREADS) {
         s_ids[j] = ids[j];
         const int k = board_find(B.keys, B.n_markers, ids[j]);
@@ -1516,6 +1531,9 @@ struct DiamondArgs {
     const int32_t* count;   // [F]                     the markers (k_finish, k_marker_refine, or one host list)
     const int32_t* ids;     // [F][max_markers]
     const float* corners;   // [F][max_markers][8]
+    const int32_t* run;     // as BoardPoseArgs
+    int family;             // the diamonds' dictionary index (read with run only)
+    int32_t id_offset;      // its id_offset: pose.fiducial_id = ids[0] + id_offset
     int32_t* n_out;         // [F]
     fid_diamond* out;       // [F][FID_MAX_DIAMONDS]
 };
@@ -1538,9 +1556,10 @@ __global__ void __launch_bounds__(DIAMOND_THREADS) k_diamond(const DiamondArgs a
     __shared__ DiamondLayout s_L;
     __shared__ int s_nd;
     const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int n = min(a.count[f], min(a.max_markers, FID_MAX_MARKERS));
+    int n = min(a.count[f], min(a.max_markers, FID_MAX_MARKERS));
     const int32_t* ids = a.ids + (size_t)f * a.max_markers;
     const float* corners = a.corners + (size_t)f * a.max_markers * 8;
+    if (a.run) family_run(a.run, f, a.family, &ids, &corners, &n);
     const FrameImg gray{a.src + (size_t)f * a.frame_stride, a.row_stride, a.enc};
     for (int c = tid; c < 8 * n; c += DIAMOND_THREADS) s_wc[c] = corners[c];
     if (tid == 0) s_L = a.layout;
@@ -1610,7 +1629,7 @@ __global__ void __launch_bounds__(DIAMOND_THREADS) k_diamond(const DiamondArgs a
         fid_diamond r{};
         for (int j = 0; j < 4; j++) r.ids[j] = ids[s_dia[4 * k + j]];
         for (int j = 0; j < 8; j++) r.corners[j] = s_xy[8 * k + j];
-        r.pose.fiducial_id = r.ids[0];
+        r.pose.fiducial_id = r.ids[0] + a.id_offset;
         if (a.has_cam) {
             PoseOut po;
             solve_marker_pose(r.corners, a.cam, s_L.square_length, (double)s_L.square_length, &po);
@@ -1656,6 +1675,7 @@ struct DictMergeArgs {
     int32_t* out_ids;          // [F][max_markers]
     float* out_corners;        // [F][max_markers][8]
     int32_t* out_dict;         // [F][max_markers]
+    int32_t* out_run;          // [F][FID_MAX_DICTIONARIES + 1]: dictionary d's markers are out_run[d] .. out_run[d + 1] - 1
     fid_transform* out_tf;     // [F][max_markers]
     struct fid_pose_hypotheses* out_hyp;  // [F][max_markers] or nullptr
     Counters* counters;
@@ -1679,6 +1699,7 @@ __global__ void __launch_bounds__(DICT_MERGE_THREADS) k_dict_merge(const DictMer
         }
         s_off[a.n_dicts] = total;
         a.out_count[f] = total;
+        for (int d = 0; d <= a.n_dicts; d++) a.out_run[(size_t)f * (FID_MAX_DICTIONARIES + 1) + d] = min(s_off[d], total);
     }
     __syncthreads();
     const int n = s_off[a.n_dicts];

@@ -267,9 +267,17 @@ class Detector:
         _lib.check(self.lib.fid_last_pose_hypotheses(self.h, max_markers, C.byref(nf), C.cast(out, C.c_void_p)), "fid_last_pose_hypotheses")
         return out
 
-    def set_boards(self, boards):
+    @staticmethod
+    def _families(families, n):
+        fam = np.ascontiguousarray(families, np.int32).reshape(-1)
+        if len(fam) != n:
+            raise ValueError("one family per board: %d boards, %d families" % (n, len(fam)))
+        return fam
+
+    def set_boards(self, boards, families=None):
         """fid_set_boards: a list of fiducials_b200.board.Board (empty = off).  Batches submitted with a camera from now on also
-        solve one pose per (frame, board)."""
+        solve one pose per (frame, board).  families: one dictionary index per board (fid_set_family_boards), which a
+        multi-dictionary handle needs; None leaves the boards without a family."""
         boards = list(boards)
         keep = [(np.ascontiguousarray(b.ids, np.int32), np.ascontiguousarray(b.obj_points, np.float32)) for b in boards]
         arr = (_lib.fid_board * max(len(keep), 1))()
@@ -277,7 +285,11 @@ class Detector:
             arr[i].n_markers = len(ids)
             arr[i].ids = ids.ctypes.data
             arr[i].obj_points = obj.ctypes.data
-        _lib.check(self.lib.fid_set_boards(self.h, len(keep), C.cast(arr, C.c_void_p)), "fid_set_boards")
+        if families is None:
+            _lib.check(self.lib.fid_set_boards(self.h, len(keep), C.cast(arr, C.c_void_p)), "fid_set_boards")
+        else:
+            fam = self._families(families, len(keep))
+            _lib.check(self.lib.fid_set_family_boards(self.h, len(keep), C.cast(arr, C.c_void_p), fam.ctypes.data_as(C.c_void_p)), "fid_set_family_boards")
         self.n_boards = len(keep)
 
     def board_poses(self, ids, corners, K, D):
@@ -300,9 +312,10 @@ class Detector:
         _lib.check(self.lib.fid_last_board_poses(self.h, nb.value, C.byref(nf), C.byref(nb), C.cast(out, C.c_void_p)), "fid_last_board_poses")
         return [[out[f * nb.value + b] for b in range(nb.value)] for f in range(nf.value)]
 
-    def set_charuco_boards(self, boards):
+    def set_charuco_boards(self, boards, families=None):
         """fid_set_charuco_boards: a list of fiducials_b200.board.CharucoBoard (empty = off).  Batches submitted from now on also
-        find each board's chessboard corners (and, with a camera, its pose)."""
+        find each board's chessboard corners (and, with a camera, its pose).  families: as set_boards
+        (fid_set_family_charuco_boards)."""
         boards = list(boards)
         arr = (_lib.fid_charuco_board * max(len(boards), 1))()
         keep = []
@@ -313,7 +326,12 @@ class Detector:
             arr[i].square_length, arr[i].marker_length = b.square_length, b.marker_length
             arr[i].legacy_pattern, arr[i].ids = int(b.legacy), ids.ctypes.data
             arr[i].min_markers, arr[i].check_markers = b.min_markers, int(b.check_markers)
-        _lib.check(self.lib.fid_set_charuco_boards(self.h, len(boards), C.cast(arr, C.c_void_p)), "fid_set_charuco_boards")
+        if families is None:
+            _lib.check(self.lib.fid_set_charuco_boards(self.h, len(boards), C.cast(arr, C.c_void_p)), "fid_set_charuco_boards")
+        else:
+            fam = self._families(families, len(boards))
+            _lib.check(self.lib.fid_set_family_charuco_boards(self.h, len(boards), C.cast(arr, C.c_void_p), fam.ctypes.data_as(C.c_void_p)),
+                       "fid_set_family_charuco_boards")
         self.charuco_boards = boards
 
     def _charuco_split(self, recs, cids, cxy):
@@ -415,14 +433,18 @@ class Detector:
             out.append((ri[f, :r].copy(), rb[f, :r].copy(), before, left))
         return out
 
-    def set_diamonds(self, square_length, marker_length=None, min_markers=2, check_markers=True):
+    def set_diamonds(self, square_length, marker_length=None, min_markers=2, check_markers=True, family=None):
         """fid_set_diamonds: the ChArUco diamond geometry (square_length=None turns diamonds off).  Batches submitted from now on also
-        find each frame's diamonds (and, with a camera, their poses)."""
+        find each frame's diamonds (and, with a camera, their poses).  family: the dictionary index of the diamonds' markers
+        (fid_set_family_diamonds), which a multi-dictionary handle needs; None sets them without a family."""
         p = _lib.fid_diamond_params()
         if square_length is not None:
             p.enable, p.square_length, p.marker_length = 1, square_length, marker_length
             p.min_markers, p.check_markers = int(min_markers), int(bool(check_markers))
-        _lib.check(self.lib.fid_set_diamonds(self.h, C.byref(p)), "fid_set_diamonds")
+        if family is None:
+            _lib.check(self.lib.fid_set_diamonds(self.h, C.byref(p)), "fid_set_diamonds")
+        else:
+            _lib.check(self.lib.fid_set_family_diamonds(self.h, C.byref(p), int(family)), "fid_set_family_diamonds")
 
     @staticmethod
     def _diamond_split(recs):
@@ -546,14 +568,16 @@ class FiducialsNode:
             self.det.set_pose_hypotheses(True)
         # one pose per marker board (new, no reference counterpart): with boards (fiducials_b200.board.Board) the pose results carry
         # an extra attribute `board_poses` = [fid_board_pose record per board, in board order]; their message fields are unchanged
-        self.boards = list(boards)
+        # with `dictionaries`, an entry may be (board, family): the board's markers are those of that entry of the node's list (0 =
+        # `dictionary`), which a multi-dictionary node needs for every board, ChArUco board and the diamonds
+        self.boards, families = _with_families(boards)
         if self.boards:
-            self.det.set_boards(self.boards)
+            self.det.set_boards(self.boards, families)
         # ChArUco boards (new, no reference counterpart): with charuco_boards (fiducials_b200.board.CharucoBoard) the pose results
         # carry an extra attribute `charuco` = [(fid_charuco_result, corner ids, corners [n, 2]) per board, in board order]
-        self.charucoBoards = list(charuco_boards)
+        self.charucoBoards, families = _with_families(charuco_boards)
         if self.charucoBoards:
-            self.det.set_charuco_boards(self.charucoBoards)
+            self.det.set_charuco_boards(self.charucoBoards, families)
         # recovery of missed board markers (new, no reference counterpart): refine_markers = (min_rep_distance, error_correction_rate,
         # check_all_orders) runs cv2's refineDetectedMarkers against the boards after detection; the recovered markers are reported
         # like any other marker, and the results carry `recovered` = [(fiducial_id, board)] (board b, or FID_MAX_BOARDS + c for
@@ -563,10 +587,15 @@ class FiducialsNode:
             self.det.set_marker_refinement(*refine_markers)
             self.det.set_batch_marker_refinement(True)
         # ChArUco diamonds (new, no reference counterpart): diamonds = (square_length, marker_length) finds cv2's detectDiamonds among
-        # the markers; the pose results carry `diamonds` = (ids [k, 4], corners [k, 4, 2], fid_diamond records with the poses)
+        # the markers; the pose results carry `diamonds` = (ids [k, 4], corners [k, 4, 2], fid_diamond records with the poses);
+        # (square_length, marker_length, family) binds them to a family as the boards above
         self.diamondGeometry = diamonds
         if diamonds is not None:
-            self.det.set_diamonds(*diamonds)
+            self.det.set_diamonds(diamonds[0], diamonds[1], family=diamonds[2] if len(diamonds) > 2 else None)
+        # with several dictionaries the board stages read each family's markers in the one-frame batch (the stand-alone calls take
+        # lists without a family); poseEstimateCallback then publishes that batch's records
+        self._batchStages = len(self.dictSpecs) > 1 and bool(self.boards or self.charucoBoards or diamonds is not None)
+        self._stageRecords = (None, None, None)
         self._recovered = []
         self._last_frame = None  # the frame of the last imageCallback, for the ChArUco corners of poseEstimateCallback
         self.haveCamInfo = False
@@ -605,6 +634,15 @@ class FiducialsNode:
                 self.ids, self.corners = ids[0, :n].copy(), corners[0, :n].copy()
                 idx, brd, _, _ = self.det.last_marker_refinement()[0]
                 self._recovered = self._recovered_of(self.ids, idx, brd)
+            elif self._batchStages:
+                cam = (self.K, self.D, self.fiducial_len, self.fiducialLens) if self.haveCamInfo and self.doPoseEstimation else ()
+                counts, ids, corners, _ = self.det.detect_pose_batch(np.ascontiguousarray(bgr, np.uint8)[None], *cam)
+                n = int(counts[0])
+                self.ids, self.corners = ids[0, :n].copy(), corners[0, :n].copy()
+                self.dictIdx = self.det.last_dict_indices()[0, :n].copy()
+                self._stageRecords = (self.det.last_board_poses()[0] if self.boards and cam else None,
+                                      self.det.last_charuco()[0] if self.charucoBoards else None,
+                                      self.det.last_diamonds()[0] if self.diamondGeometry is not None else None)
             elif len(self.dictSpecs) > 1:
                 self.ids, self.corners, self.dictIdx = self.det.detect_multi_dict(bgr)
             else:
@@ -660,9 +698,12 @@ class FiducialsNode:
         try:
             tfs = self._per_dictionary(lambda i, c, ln: self.det.pose(i, c, self.K, self.D, ln, self.fiducialLens))
             hyps = self._per_dictionary(lambda i, c, ln: self.det.pose_hypotheses(i, c, self.K, self.D, ln, self.fiducialLens)) if self.poseHypotheses else None
-            boards = self.det.board_poses(self.ids, self.corners, self.K, self.D) if self.boards else None
-            charuco = self.det.charuco(self._last_frame, self.ids, self.corners, self.K, self.D) if self.charucoBoards and self._last_frame is not None else None
-            diamonds = self.det.diamonds(self._last_frame, self.ids, self.corners, self.K, self.D) if self.diamondGeometry is not None and self._last_frame is not None else None
+            if self._batchStages:
+                boards, charuco, diamonds = self._stageRecords
+            else:
+                boards = self.det.board_poses(self.ids, self.corners, self.K, self.D) if self.boards else None
+                charuco = self.det.charuco(self._last_frame, self.ids, self.corners, self.K, self.D) if self.charucoBoards and self._last_frame is not None else None
+                diamonds = self.det.diamonds(self._last_frame, self.ids, self.corners, self.K, self.D) if self.diamondGeometry is not None and self._last_frame is not None else None
         except _lib.FidError:
             return fta
         if self.vis_msgs:  # :403, :462-478: vision_msgs/Detection2DArray instead of FiducialTransformArray
@@ -730,6 +771,16 @@ class FiducialsNode:
                 fta.recovered = self._recovered_of(ids[f, : int(counts[f])], refined[f][0], refined[f][1])
             out.append(fta)
         return out
+
+
+def _with_families(items):
+    """Boards given as board or (board, family): (boards, families), families None when no entry names one (the setters without a
+    family), else one per board with 0 for a bare board."""
+    items = list(items)
+    if not any(isinstance(b, tuple) for b in items):
+        return items, None
+    pairs = [b if isinstance(b, tuple) else (b, 0) for b in items]
+    return [b for b, _ in pairs], [int(f) for _, f in pairs]
 
 
 def _to_msg(t) -> FiducialTransform:

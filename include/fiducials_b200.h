@@ -372,9 +372,28 @@ typedef struct fid_dictionary_spec {
  * fid_create applies to fid_params.dictionary: FID_ERR_UNSUPPORTED / FID_ERR_INVALID_ARG otherwise, also for a length that is
  * negative or not finite or an offset with which id + id_offset overflows int32, each with the handle unchanged.  A handle is in
  * multi-dictionary mode when the list has more than one entry or entry 0 has an offset or a length; the batch calls then detect
- * with every dictionary.  Marker boards, ChArUco boards, batch marker refinement and diamonds are refused (FID_ERR_UNSUPPORTED,
- * nothing changed) in that mode, in both directions.  Not while batches are in flight. */
+ * with every dictionary.  Batch marker refinement, and boards, ChArUco boards and diamonds set without a family (fid_set_boards,
+ * fid_set_charuco_boards, fid_set_diamonds), are refused (FID_ERR_UNSUPPORTED, nothing changed) in that mode, in both directions.
+ * With boards bound to families (fid_set_family_*), a new list is accepted when every bound index still names an entry of it;
+ * FID_ERR_INVALID_ARG, with the handle unchanged, when a bound index would not, or when a bound ChArUco board has more markers than
+ * its new family's dictionary.  Not while batches are in flight. */
 int fid_set_dictionaries(fid_detector* h, int n, const fid_dictionary_spec* specs);
+/* Boards bound to dictionary families (NEW): fid_set_boards, fid_set_charuco_boards and fid_set_diamonds, each board (or the
+ * diamonds) bound to an entry of the handle's dictionary list, dict_index in fid_set_dictionaries order.  Raw ids repeat across
+ * families (DICT_4X4_50 id 3 and DICT_5X5_1000 id 3 are different markers), so in multi-dictionary mode a stage bound to family k
+ * reads that family's markers alone, in list order: what a cv2 4.13 user gets by running Board::matchImagePoints + solvePnP,
+ * CharucoDetector(CharucoBoard(..., dicts[k], ids)).detectBoard and CharucoDetector(CharucoBoard((3, 3), ..., dicts[k]))
+ * .detectDiamonds on corners[di == k], ids[di == k] of detectMarkersMultiDict, with family k's detector parameters.  A diamond's
+ * pose.fiducial_id is ids[0] + family k's id_offset (its ids stay raw).  The batch calls (fid_detect_pose_batch, fid_submit_batch /
+ * fid_collect_batch) run the stages after the merge and fid_last_board_poses / fid_last_charuco / fid_last_diamonds return them as
+ * usual; fid_detect_multi_dict runs the ChArUco stage as fid_detect does.  fid_estimate_board_poses, fid_detect_charuco,
+ * fid_detect_diamonds and fid_refine_detected_markers return FID_ERR_UNSUPPORTED in multi-dictionary mode (their lists carry no
+ * family), and fid_detect there runs no board stage.  Each call accepts what its counterpart accepts, plus
+ * 0 <= dict_index < the number of entries (FID_ERR_INVALID_ARG, handle unchanged, otherwise); on a single-dictionary handle index 0
+ * gives exactly the counterpart's outputs. */
+int fid_set_family_boards(fid_detector* h, int n_boards, const fid_board* boards, const int32_t* dict_index);
+int fid_set_family_charuco_boards(fid_detector* h, int n_boards, const fid_charuco_board* boards, const int32_t* dict_index);
+int fid_set_family_diamonds(fid_detector* h, const fid_diamond_params* params, int32_t dict_index);
 /* detectMarkersMultiDict for one frame (fid_detect's arguments): ids, corners and dict_indices (may be NULL) [n], max_markers a
  * total over all dictionaries (FID_ERR_CAPACITY with the first max_markers written beyond it).  fid_detect stays detectMarkers
  * with dictionary 0 alone, as cv2's detectMarkers on a detector with several dictionaries. */
