@@ -479,8 +479,11 @@ extern "C" int fid_create(const fid_params* params, int device, int max_width, i
     CKH(cudaGetDeviceProperties(&prop, device));
     h->sm_count = prop.multiProcessorCount;
     const size_t px = (size_t)max_width * max_height * max_batch;
-    // Worst case measured on uniform-noise frames with the reference's 13 scales: 4.9 start cracks and
-    // 3.6 in-range contour points per pixel (typical marker scenes: 0.3 and 0.4).
+    // Start cracks: at most one left and one right crack per two pixels of a row and plane (halo_row_starts), i.e.
+    // n_scales / 2 per pixel and side -- 6.5 with the reference's 13 scales.  Uniform noise gives 1.6, marker scenes 0.15;
+    // a 1-pixel checkerboard or dither reaches the bound.  The queue holds 3 per pixel and side: a chunk with more is
+    // walked again from its stored planes in groups of scales that fit (k_rescan_starts), so its result does not change.
+    // In-range contour points: 3.6 per pixel on uniform noise (marker scenes 0.4); past the capacity, FID_ERR_CAPACITY.
     h->max_starts = (unsigned int)std::min<size_t>(px * 6 + 65536, 0x7fffffffu);
     h->max_chains = (unsigned int)std::min<size_t>((size_t)max_batch * 65536, 0x7fffffffu);
     h->max_points = (unsigned int)std::min<size_t>(px * 4 + 65536, 0x7fffffffu);
@@ -942,6 +945,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         seg_enc = FID_ENC_MONO8;
     }
     const int W = gs.W, H = gs.H;
+    bool padded_starts = false;  // the tensor-core kernel queues start cracks in blocks padded with null records
     {  // threshold stage: gray + 13 adaptive thresholds -> halo tiles + start cracks
         bool fast = P.n_scales == 13;
         for (int i = 0; i < P.n_scales; i++) fast = fast && P.win[i] == 3 + 4 * i;
@@ -970,6 +974,7 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
             CUtensorMap tmap;
             memset(&tmap, 0, sizeof(tmap));
             static const bool tma_off = getenv("FID_THRESH_TMA") && atoi(getenv("FID_THRESH_TMA")) == 0;  // debugging switch
+            padded_starts = true;
             a.use_tma = (!tma_off && seg_enc != FID_ENC_MONO8 && make_bgr_tensor_map(&tmap, seg_src, W, H, nf, gs.bgr_row_stride, gs.bgr_frame_stride)) ? 1 : 0;
             const long long total = (long long)a.tiles_x * a.tiles_y * nf;
             const int grid = (int)std::min<long long>(total, h->sm_count);
@@ -1058,23 +1063,52 @@ static int enqueue_pipeline(fid_detector* h, Slot& s, cudaStream_t st, int nf, c
         a.g = gs;
         a.min_len = min_len;
         a.max_len = max_len;
-        for (int r = 0; r < N_WALK_ROUNDS; r++) {
-            CK(cudaEventRecord(s.ev_round[r], st));
-            if (r >= h->walk_rounds) continue;
-            a.round = r;
-            a.budget = h->walk_budget[r];
-            a.persistent = h->walk_persist[r];
-            a.q_in = r > 0 ? s.d_queue[(r - 1) & 1] : nullptr;
-            a.q_out = s.d_queue[r & 1];
-            a.chunk = r == 0 ? 256u : 32u;
-            a.refill_min = h->walk_refill;
-            a.pass_steps = h->walk_pass;
-            static const int wb2 = getenv("FID_WALK_BLOCKS_R2") ? atoi(getenv("FID_WALK_BLOCKS_R2")) : 4, wb3 = getenv("FID_WALK_BLOCKS_R3") ? atoi(getenv("FID_WALK_BLOCKS_R3")) : 4;
-            const int blocks = r == 0 ? h->sm_count * 8 : (r == 1 ? h->sm_count * 8 : h->sm_count * (r == 2 ? wb2 : wb3));
-            launch_prio(k_walk, dim3(blocks), dim3(256), 0, st, r == 0 ? 1 : (r == 1 ? 2 : 3), a);
-            launches++;
-        }
+        // the rounds over the start queue of the threshold kernel (replay_group -1) or of one scale group of the replay
+        auto walk_rounds = [&](int replay_group, bool timed) {
+            a.replay_group = replay_group;
+            for (int r = 0; r < N_WALK_ROUNDS; r++) {
+                if (timed) CK(cudaEventRecord(s.ev_round[r], st));
+                if (r >= h->walk_rounds) continue;
+                a.round = r;
+                a.budget = h->walk_budget[r];
+                a.persistent = h->walk_persist[r];
+                a.q_in = r > 0 ? s.d_queue[(r - 1) & 1] : nullptr;
+                a.q_out = s.d_queue[r & 1];
+                a.chunk = r == 0 ? 256u : 32u;
+                a.refill_min = h->walk_refill;
+                a.pass_steps = h->walk_pass;
+                static const int wb2 = getenv("FID_WALK_BLOCKS_R2") ? atoi(getenv("FID_WALK_BLOCKS_R2")) : 4, wb3 = getenv("FID_WALK_BLOCKS_R3") ? atoi(getenv("FID_WALK_BLOCKS_R3")) : 4;
+                const int blocks = r == 0 ? h->sm_count * 8 : (r == 1 ? h->sm_count * 8 : h->sm_count * (r == 2 ? wb2 : wb3));
+                launch_prio(k_walk, dim3(blocks), dim3(256), 0, st, r == 0 ? 1 : (r == 1 ? 2 : 3), a);
+                launches++;
+            }
+            return FID_OK;
+        };
+        if (int rc = walk_rounds(-1, true)) return rc;
         CK(cudaEventRecord(s.ev_round[N_WALK_ROUNDS], st));
+        // start-queue replay (kernels_contour.cuh, k_rescan_starts): scale groups of at most `per_group` planes, so that a group's
+        // start cracks -- at most ceil(W / 2) per row, plane and side -- fit the queue's max_starts / 2 per side.  Not enqueued
+        // where the planes of one chunk cannot hold more cracks than that and the queue holds no padding.
+        const size_t per_plane = (size_t)((W + 1) / 2) * H * nf, cap = h->max_starts / 2;
+        if (padded_starts || per_plane * P.n_scales > cap) {
+            const int per_group = (int)std::max<size_t>(1, std::min<size_t>(P.n_scales, cap / per_plane));
+            RescanArgs ra{};
+            ra.halo = s.d_halo;
+            ra.starts = s.d_starts;
+            ra.counters = s.d_counters;
+            ra.max_starts = h->max_starts;
+            ra.prune = h->start_prune ? h->d_prune : nullptr;
+            ra.g = gs;
+            ra.n_frames = nf;
+            for (int g0 = 0, grp = 0; g0 < P.n_scales; g0 += per_group, grp++) {
+                ra.s_lo = g0;
+                ra.s_hi = std::min(P.n_scales, g0 + per_group);
+                ra.group = grp;
+                launch_prio(k_rescan_starts, dim3(h->sm_count * 8), dim3(256), 0, st, 1, ra);
+                launches++;
+                if (int rc = walk_rounds(grp, false)) return rc;
+            }
+        }
     }
     CK(cudaEventRecord(s.ev[ST_EMIT], st));
     {  // emit

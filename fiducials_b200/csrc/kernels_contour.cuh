@@ -31,7 +31,13 @@ struct Counters {
     unsigned int approx_work;  // k_approx_warp work counter
     unsigned int n_first;      // selected candidates of the chunk (k_sort_group -> k_identify_first work list)
     unsigned int n_retry;      // candidates whose first identification attempt failed (-> k_identify_retry work list)
+    unsigned int n_rescan[FID_MAX_SCALES][2];  // start cracks of each scale group of a start-queue replay (k_rescan_starts), per side
 };
+
+// The start queue overflowed: n_starts counts every start crack the threshold kernel found, also those it had no room for.
+__device__ __forceinline__ bool start_queue_overflowed(const Counters* c, unsigned int max_starts) {
+    return c->n_starts[0] > max_starts / 2 || c->n_starts[1] > max_starts / 2;
+}
 
 struct WalkRec {       // a bidirectional border walk suspended between rounds (contour_walk.cuh, WalkState2)
     uint32_t xy0;      // start pixel
@@ -113,6 +119,7 @@ struct WalkArgs {
     Counters* counters;
     unsigned int max_starts, max_chains, max_points, max_queue, max_segs;
     int round;                // 0 = items are start cracks
+    int replay_group;         // -1: the walk of the threshold kernel's queue; >= 0: a scale group of the start-queue replay
     FrameGeom g;
     int min_len, max_len, budget;
     int persistent;
@@ -292,13 +299,17 @@ __device__ __forceinline__ void walk_side(const WalkArgs& a, const StepTabs<uint
 }
 
 __global__ void __launch_bounds__(256) k_walk(const WalkArgs a) {
+    if (a.replay_group >= 0 && !start_queue_overflowed(a.counters, a.max_starts)) return;
     __shared__ __align__(16) uint8_t s_tabs[2 * FID_LUT_SIZE];
     const StepTabs<uint8_t> tabs = stage_step_tables(a.step_bytes, s_tabs);
     unsigned int nL, nR;
     if (a.round == 0) {
-        nL = a.counters->n_starts[0];
-        nR = a.counters->n_starts[1];
+        const unsigned int* n0 = a.replay_group >= 0 ? a.counters->n_rescan[a.replay_group] : a.counters->n_starts;
+        nL = n0[0];
+        nR = n0[1];
         const unsigned int cap = a.max_starts / 2;
+        // a scale group larger than the queue (the walk stage never forms one): its excess cracks were dropped
+        if (a.replay_group >= 0 && (nL > cap || nR > cap) && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(&a.counters->overflow, 1u);
         nL = nL < cap ? nL : cap;
         nR = nR < cap ? nR : cap;
     } else {
@@ -316,6 +327,76 @@ __global__ void __launch_bounds__(256) k_walk(const WalkArgs a) {
     if (!nR) wL = total_warps;
     if (nL) walk_side<false>(a, tabs, nL, 0, wL);
     if (nR) walk_side<true>(a, tabs, nR, wL, total_warps - wL);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Start-queue replay.  A plane holds at most one left and one right start crack per two pixels of a row
+// (halo_row_starts: a left crack needs mid & ~mid_l), so n_scales / 2 per pixel and side in all -- 6.5 with the
+// default 13 windows -- while the queue holds 3 (fid_create).  Uniform noise and camera scenes stay near 1.6; a
+// 1-pixel checkerboard or dither reaches the bound on every plane.  When the threshold kernel had to drop start
+// cracks, the walk's chains are discarded and the start cracks are found again from the stored halo planes, one
+// group of scales at a time, each group small enough that its cracks provably fit (fid_api.cu, walk stage); every
+// group is walked by the usual rounds.  Without an overflow every replay launch returns at once.
+// ---------------------------------------------------------------------------------------------------
+struct RescanArgs {
+    const uint32_t* halo;
+    StartRec* starts;
+    Counters* counters;
+    unsigned int max_starts;
+    const uint32_t* prune;  // start_prune_table.h on the device, or null
+    FrameGeom g;
+    int n_frames;
+    int s_lo, s_hi, group;  // scales [s_lo, s_hi) form scale group `group`
+};
+
+// one warp per halo tile (lane = tile row), grid-stride over the tiles of the chunk
+__global__ void __launch_bounds__(256) k_rescan_starts(const RescanArgs a) {
+    Counters* c = a.counters;
+    if (!start_queue_overflowed(c, a.max_starts)) return;
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        // the walk rounds of the previous group (or of the threshold kernel's queue) have finished: their queues are reset, and
+        // before the first group, their chains -- incomplete, since start cracks were dropped
+        for (int r = 0; r < FID_WALK_MAX_ROUNDS; r++) c->n_q[r][0] = c->n_q[r][1] = c->work[r][0] = c->work[r][1] = 0u;
+        if (a.group == 0) {
+            c->n_chains = c->n_points = c->n_segs = 0u;
+            atomicAnd(&c->overflow, ~(1u | 2u | 4u | 64u));
+        }
+    }
+    const int lane = threadIdx.x & 31;
+    const unsigned int tiles_per_frame = (unsigned int)(a.g.halo_tpr * a.g.halo_tiles_y), n_tiles = tiles_per_frame * (unsigned int)a.n_frames;
+    const unsigned int cap = a.max_starts / 2;
+    for (unsigned int t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < n_tiles; t += (gridDim.x * blockDim.x) >> 5) {
+        const unsigned int f = t / tiles_per_frame, pt = t - f * tiles_per_frame;
+        const uint32_t* tile = a.halo + (size_t)f * a.g.halo_frame_stride + (size_t)pt * 32;
+        for (int s = a.s_lo; s < a.s_hi; s++) {
+            const uint32_t mid = tile[(size_t)s * a.g.halo_scale_stride + lane];
+            const uint32_t up = __shfl_up_sync(0xffffffffu, mid, 1), dn = __shfl_down_sync(0xffffffffu, mid, 1);
+            uint32_t L = 0, R = 0;
+            if (lane >= 1 && lane <= FID_HALO_T && mid) halo_row_starts(up, mid, dn, &L, &R);
+            if (a.prune && (L | R)) halo_prune_starts(up, mid, dn, &L, &R, a.prune);
+            const unsigned int cnt = (unsigned int)__popc(L) | ((unsigned int)__popc(R) << 16);  // both counts in one scan
+            unsigned int incl = cnt;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const unsigned int v = __shfl_up_sync(0xffffffffu, incl, d);
+                if (lane >= d) incl += v;
+            }
+            const unsigned int tot = __shfl_sync(0xffffffffu, incl, 31);
+            if (!tot) continue;
+            unsigned int bl = 0, br = 0;
+            if (lane == 31) {
+                bl = (tot & 0xffffu) ? atomicAdd(&c->n_rescan[a.group][0], tot & 0xffffu) : 0u;
+                br = (tot >> 16) ? atomicAdd(&c->n_rescan[a.group][1], tot >> 16) : 0u;
+            }
+            unsigned int pl = __shfl_sync(0xffffffffu, bl, 31) + ((incl - cnt) & 0xffffu);
+            unsigned int pr = __shfl_sync(0xffffffffu, br, 31) + ((incl - cnt) >> 16);
+            const uint32_t rec = start_rec_pack(t, (uint32_t)s, (uint32_t)lane, 0u);
+            for (; L; L &= L - 1, pl++)
+                if (pl < cap) a.starts[pl].v = rec | (uint32_t)(__ffs(L) - 1);
+            for (; R; R &= R - 1, pr++)
+                if (pr < cap) a.starts[a.max_starts - 1 - pr].v = rec | (uint32_t)(__ffs(R) - 1);
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------
