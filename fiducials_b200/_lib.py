@@ -244,6 +244,7 @@ EXPORTS = [
     "fid_map_load", "fid_map_links", "fid_map_add_links", "fid_map_update", "fid_map_update_sequence", "fid_map_update_frames", "fid_map_update_frames_async", "fid_map_sync", "fid_map_entries", "fid_map_export", "fid_map_merge", "fid_map_export_device",
     "fid_map_merge_device", "fid_map_merge_device_async", "fid_map_export_async", "fid_map_stream", "fid_map_merged_entries", "fid_map_adopt_merged", "fid_map_add_fiducial", "fid_map_refine_default_params", "fid_map_refine",
     "fid_jpeg_create", "fid_jpeg_destroy", "fid_jpeg_decode_batch", "fid_jpeg_sync", "fid_jpeg_stream", "fid_jpeg_last_stats", "fid_calibrate_camera",
+    "fid_calibrate_camera_ro",
 ]
 
 _lib = None
@@ -346,6 +347,7 @@ def load():
     lib.fid_jpeg_last_stats.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]
     lib.fid_calibrate_camera.argtypes = [i32, i32, vp, vp, vp, i32, i32, C.POINTER(fid_camera), i32, C.POINTER(fid_calib_criteria), C.POINTER(fid_calib_result), vp, vp,
                                          vp, vp, C.POINTER(fid_calib_stats)]
+    lib.fid_calibrate_camera_ro.argtypes = lib.fid_calibrate_camera.argtypes + [i32, vp, vp, C.POINTER(C.c_int)]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError if the build lost a symbol
     _lib = lib

@@ -201,7 +201,8 @@ FID_HD void calib_init_intrinsics(const double t[5], int width, int height, doub
 
 // One point: residual e = projection - image point, and its Jacobian over the 9 intrinsics and the view's 6 extrinsics
 // (cvProjectPoints2Internal's dpdf / dpdc / dpdk / dpdr / dpdt).
-FID_HD void calib_point(const float* o, const float* m, const double in[9], double aspect, const double R[9], const double* dRdr, const double p[6],
+template <class T>
+FID_HD void calib_point(const T* o, const float* m, const double in[9], double aspect, const double R[9], const double* dRdr, const double p[6],
                         double e[2], double Ji[2][9], double Je[2][6]) {
     const Camera cam = calib_camera(in);
     double uv[2];
@@ -229,7 +230,8 @@ FID_HD void calib_point(const float* o, const float* m, const double in[9], doub
 }
 
 // Stage 4, one view: the blocks U, W, V, gi, ge and the cost at intrinsics `in` and extrinsics p (layout CALIB_*).
-FID_HD void calib_view_eval(int n, const float* obj, const float* img, const double in[9], double aspect, const double p[6], double* blk) {
+template <class T>
+FID_HD void calib_view_eval(int n, const T* obj, const float* img, const double in[9], double aspect, const double p[6], double* blk) {
     double R[9], dRdr[27];
     rodrigues_v2m(p, R, dRdr);
     auto point = [&](int i, double e[2], double Ji[2][9], double Je[2][6]) { calib_point(obj + 3 * i, img + 2 * i, in, aspect, R, dRdr, p, e, Ji, Je); };
@@ -329,6 +331,20 @@ FID_HD void calib_solve_intrinsics(const double U[45], const double g[9], const 
         if (!mask[a]) d[a] = 0.0;
 }
 
+// One view's cost sum e^2 at intrinsics `in`, extrinsics p and object points obj.
+template <class T>
+FID_HD double calib_view_cost(int n, const T* obj, const float* img, const double in[9], double aspect, const double p[6]) {
+    double R[9];
+    rodrigues_v2m(p, R, nullptr);
+    double c;
+    board_sum<1>(n, [&](int i, double v[1]) {
+        double e[2];
+        calib_point(obj + 3 * i, img + 2 * i, in, aspect, R, nullptr, p, e, nullptr, nullptr);
+        v[0] = e[0] * e[0] + e[1] * e[1];
+    }, &c);
+    return c;
+}
+
 // Stage 4, one view: the back-substituted extrinsic step, the trial parameters p = pp - d and, at the trial intrinsics `in`,
 // out = {cost, |p - pp|^2, |pp|^2}.
 FID_HD void calib_view_trial(int n, const float* obj, const float* img, const double in[9], double aspect, const double* blk, const double* sch,
@@ -347,15 +363,7 @@ FID_HD void calib_view_trial(int n, const float* obj, const float* img, const do
         dn += (p[j] - pp[j]) * (p[j] - pp[j]);
         pn += pp[j] * pp[j];
     }
-    double R[9];
-    rodrigues_v2m(p, R, nullptr);
-    double c;
-    board_sum<1>(n, [&](int i, double v[1]) {
-        double e[2];
-        calib_point(obj + 3 * i, img + 2 * i, in, aspect, R, nullptr, p, e, nullptr, nullptr);
-        v[0] = e[0] * e[0] + e[1] * e[1];
-    }, &c);
-    out[0] = c;
+    out[0] = calib_view_cost(n, obj, img, in, aspect, p);
     out[1] = dn;
     out[2] = pn;
 }
@@ -461,6 +469,210 @@ FID_HD void calib_schur_inverse(const double U[45], const double Q[45], const in
         solve_sym<9>(S, u, x);
         for (int a = 0; a < 9; a++) Sinv[a][c] = mask[a] && mask[c] ? x[a] : 0.0;
     }
+}
+
+// ---- object release: cv::calibrateCameraRO (calibrateCameraROExtended), DESIGN.md finding 21 ---------------------------------
+// Every view holds the same n object points (the board); the parameters are the 9 intrinsics, 6 per view and the 3n board
+// coordinates, of which the 7 of point 0, of point `fixed` and z of point n - 1 stay fixed.  J^T J gains the point blocks
+// P_i = sum_v Jo^T Jo (3x3, a point enters only its own residuals), X_i = sum_v Ji^T Jo (9x3) and, per view, the cross columns
+// Y_vi = Je^T Jo (6x3).  Eliminating the views' 6x6 blocks leaves the dense system over the m = 9 + 3n intrinsics and
+// coordinates (fixed ones as identity rows): S = A - sum_v Z_v Z_v^T, Z_v = [W_v; Y_v] L_v^-T with L_v L_v^T the damped V_v,
+// r = g - sum_v Z_v h_v, h_v = L_v^-1 ge_v; the dense kernels of calib_dense.cuh factor it (the host build: a plain Cholesky).
+#define CALIB_PT_X 0   // per point: X 9x3 row-major 27
+#define CALIB_PT_P 27  // P upper 6 (xx xy xz yy yz zz)
+#define CALIB_PT_G 33  // go = sum Jo^T e 3
+#define CALIB_PT 36
+#define CALIB_FAC_L 0   // per view: L of the damped V, lower, packed row by row 21
+#define CALIB_FAC_H 21  // h = L^-1 ge 6
+#define CALIB_FAC 27
+#define CALIB_RO_MAX_POINTS 1024  // per view: m <= 3081
+#define CALIB_RO_MAX_VIEWS 4096
+
+// d (u, v) / d (X, Y, Z) of one point from its d (u, v) / d t: the point enters the camera frame as R X + t.
+FID_HD void calib_point_obj(const double Je[2][6], const double R[9], double Jo[2][3]) {
+    for (int r = 0; r < 2; r++)
+        for (int c = 0; c < 3; c++) Jo[r][c] = Je[r][3] * R[c] + Je[r][4] * R[3 + c] + Je[r][5] * R[6 + c];
+}
+
+// The release mask: coordinate c of point i is free unless it is one of point 0's, one of point `fixed`'s or z of point n - 1.
+FID_HD bool calib_ro_free(int i, int c, int n, int fixed) { return i != 0 && i != fixed && !(i == n - 1 && c == 2); }
+
+// Free parameters of a released run (the sigma^2 count): the free intrinsics, 6 per view and 3n - 7 coordinates.
+FID_HD int calib_ro_nfree(const int mask[9], int nv, int n) {
+    int k = 6 * nv + 3 * n - 7;
+    for (int a = 0; a < 9; a++) k += mask[a];
+    return k;
+}
+
+// Point i's sums over the views, in view order (layout CALIB_PT_*), at intrinsics `in`, the views' extrinsics p[6 nv] and the
+// board obj[3n]; img holds n points per view.
+FID_HD void calib_ro_point_sums(int nv, int n, int i, const double* obj, const float* img, const double in[9], double aspect, const double* p, double* out) {
+    for (int k = 0; k < CALIB_PT; k++) out[k] = 0.0;
+    for (int v = 0; v < nv; v++) {
+        double R[9], dRdr[27], e[2], Ji[2][9], Je[2][6], Jo[2][3];
+        rodrigues_v2m(p + 6 * v, R, dRdr);
+        calib_point(obj + 3 * i, img + 2 * ((size_t)n * v + i), in, aspect, R, dRdr, p + 6 * v, e, Ji, Je);
+        calib_point_obj(Je, R, Jo);
+        for (int a = 0; a < 9; a++)
+            for (int c = 0; c < 3; c++) out[CALIB_PT_X + 3 * a + c] += Ji[0][a] * Jo[0][c] + Ji[1][a] * Jo[1][c];
+        for (int a = 0, o = 0; a < 3; a++)
+            for (int b = a; b < 3; b++, o++) out[CALIB_PT_P + o] += Jo[0][a] * Jo[0][b] + Jo[1][a] * Jo[1][b];
+        for (int c = 0; c < 3; c++) out[CALIB_PT_G + c] += Jo[0][c] * e[0] + Jo[1][c] * e[1];
+    }
+}
+
+FID_HD void calib_ro_lsolve6(const double* L, const double b[6], double z[6]) {  // L z = b
+    for (int a = 0; a < 6; a++) {
+        double s = b[a];
+        for (int k = 0; k < a; k++) s -= L[a * (a + 1) / 2 + k] * z[k];
+        z[a] = s / L[a * (a + 1) / 2 + a];
+    }
+}
+FID_HD void calib_ro_ltsolve6(const double* L, const double b[6], double x[6]) {  // L^T x = b
+    for (int a = 5; a >= 0; a--) {
+        double s = b[a];
+        for (int k = a + 1; k < 6; k++) s -= L[k * (k + 1) / 2 + a] * x[k];
+        x[a] = s / L[a * (a + 1) / 2 + a];
+    }
+}
+
+// One view: the Cholesky factor L of V with its diagonal times `scale`, and h = L^-1 ge (layout CALIB_FAC_*); false on a
+// non-positive pivot.
+FID_HD bool calib_ro_view_factor(const double* blk, double scale, double* fac) {
+    double A[6][6];
+    for (int a = 0, o = 0; a < 6; a++)
+        for (int b = a; b < 6; b++, o++) A[a][b] = A[b][a] = blk[CALIB_V + o];
+    for (int a = 0; a < 6; a++) A[a][a] *= scale;
+    double* L = fac + CALIB_FAC_L;
+    for (int a = 0; a < 6; a++)
+        for (int b = 0; b <= a; b++) {
+            double s = A[a][b];
+            for (int k = 0; k < b; k++) s -= L[a * (a + 1) / 2 + k] * L[b * (b + 1) / 2 + k];
+            if (a != b) {
+                L[a * (a + 1) / 2 + b] = s / L[b * (b + 1) / 2 + b];
+            } else {
+                if (!(s > 0.0)) return false;
+                L[a * (a + 1) / 2 + a] = sqrt(s);
+            }
+        }
+    calib_ro_lsolve6(L, blk + CALIB_GE, fac + CALIB_FAC_H);
+    return true;
+}
+
+// One view's 9 intrinsic rows of Z = W L^-T (rows of fixed intrinsics 0).
+FID_HD void calib_ro_z_intrinsics(const double* blk, const double* fac, const int mask[9], double z[9][6]) {
+    for (int a = 0; a < 9; a++) {
+        const double zero[6] = {0, 0, 0, 0, 0, 0};
+        calib_ro_lsolve6(fac + CALIB_FAC_L, mask[a] ? blk + CALIB_W + 6 * a : zero, z[a]);
+    }
+}
+
+// One view's 3 rows of point i in Z = Y L^-T, Y = Je^T Jo of the point at `in`, p and the board coordinates o (rows of fixed
+// coordinates 0).
+FID_HD void calib_ro_z_point(const double* o, const float* m, const double in[9], double aspect, const double p[6], const double* fac, int i, int n, int fixed,
+                             double z[3][6]) {
+    double R[9], dRdr[27], e[2], Je[2][6], Jo[2][3];
+    rodrigues_v2m(p, R, dRdr);
+    calib_point(o, m, in, aspect, R, dRdr, p, e, nullptr, Je);
+    calib_point_obj(Je, R, Jo);
+    for (int c = 0; c < 3; c++) {
+        double y[6];
+        const bool f = calib_ro_free(i, c, n, fixed);
+        for (int j = 0; j < 6; j++) y[j] = f ? Je[0][j] * Jo[0][c] + Je[1][j] * Jo[1][c] : 0.0;
+        calib_ro_lsolve6(fac + CALIB_FAC_L, y, z[c]);
+    }
+}
+
+// Entry (a, b), a >= b, of A = [U X; X^T P] (the diagonal times `scale`) over the m = 9 + 3n parameters; the rows and columns of
+// fixed parameters, and the rows past m up to a padded size, are the identity.
+FID_HD bool calib_ro_param_free(int a, int n, int fixed, const int mask[9]) {
+    return a < 9 ? mask[a] != 0 : (a < 9 + 3 * n && calib_ro_free((a - 9) / 3, (a - 9) % 3, n, fixed));
+}
+FID_HD double calib_ro_entry(int a, int b, int n, int fixed, const int mask[9], const double U[45], const double* pts, double scale) {
+    if (!calib_ro_param_free(a, n, fixed, mask) || !calib_ro_param_free(b, n, fixed, mask)) return a == b ? 1.0 : 0.0;
+    double s;
+    if (a < 9) {
+        s = U[b * 9 - b * (b - 1) / 2 + a - b];
+    } else if (b < 9) {
+        s = pts[(size_t)CALIB_PT * ((a - 9) / 3) + CALIB_PT_X + 3 * b + (a - 9) % 3];
+    } else {
+        const int ia = (a - 9) / 3, ca = (a - 9) % 3, ib = (b - 9) / 3, cb = (b - 9) % 3;
+        if (ia != ib) return 0.0;
+        s = pts[(size_t)CALIB_PT * ia + CALIB_PT_P + cb * 3 - cb * (cb - 1) / 2 + ca - cb];
+    }
+    return a == b ? s * scale : s;
+}
+// Entry a of g = [gi; go] (0 for fixed parameters and past m).
+FID_HD double calib_ro_grad(int a, int n, int fixed, const int mask[9], const double gi[9], const double* pts) {
+    if (!calib_ro_param_free(a, n, fixed, mask)) return 0.0;
+    return a < 9 ? gi[a] : pts[(size_t)CALIB_PT * ((a - 9) / 3) + CALIB_PT_G + (a - 9) % 3];
+}
+
+// Stage 4 with released points, one view: r = ge - W^T dint - sum_i Y_i dobj_i (Y at the J's parameters in_prev, pp, obj_prev),
+// the step x = Vd^-1 r from the view's factor, p = pp - x and, at the trial parameters `in`, p and obj, out = {cost,
+// |p - pp|^2, |pp|^2}.
+FID_HD void calib_ro_view_trial(int n, const double* obj_prev, const double* obj, const double* dobj, const float* img, const double in_prev[9], const double in[9],
+                                double aspect, const double* blk, const double* fac, const double dint[9], const double pp[6], double p[6], double out[3]) {
+    double R[9], dRdr[27], t[6];
+    rodrigues_v2m(pp, R, dRdr);
+    board_sum<6>(n, [&](int i, double v[6]) {
+        double e[2], Je[2][6], Jo[2][3];
+        calib_point(obj_prev + 3 * i, img + 2 * i, in_prev, aspect, R, dRdr, pp, e, nullptr, Je);
+        calib_point_obj(Je, R, Jo);
+        const double* d = dobj + 3 * i;
+        const double jd0 = Jo[0][0] * d[0] + Jo[0][1] * d[1] + Jo[0][2] * d[2], jd1 = Jo[1][0] * d[0] + Jo[1][1] * d[1] + Jo[1][2] * d[2];
+        for (int k = 0; k < 6; k++) v[k] = Je[0][k] * jd0 + Je[1][k] * jd1;
+    }, t);
+    double r[6], z[6], x[6];
+    for (int k = 0; k < 6; k++) {
+        double s = blk[CALIB_GE + k];
+        for (int a = 0; a < 9; a++) s -= blk[CALIB_W + 6 * a + k] * dint[a];
+        r[k] = s - t[k];
+    }
+    calib_ro_lsolve6(fac + CALIB_FAC_L, r, z);
+    calib_ro_ltsolve6(fac + CALIB_FAC_L, z, x);
+    double dn = 0.0, pn = 0.0;
+    for (int j = 0; j < 6; j++) {
+        p[j] = pp[j] - x[j];
+        dn += (p[j] - pp[j]) * (p[j] - pp[j]);
+        pn += pp[j] * pp[j];
+    }
+    out[0] = calib_view_cost(n, obj, img, in, aspect, p);
+    out[1] = dn;
+    out[2] = pn;
+}
+
+// Stage 5 with released points, one view: the standard deviations of its rvec and tvec, diag(V^-1 + V^-1 B^T S^-1 B V^-1)
+// sigma^2 from the undamped factor L (V = L L^T) and M = Z^T S^-1 Z (6x6, Z = B L^-T; M = T^T T with T = L_S^-1 Z).
+FID_HD void calib_ro_view_std(const double* fac, const double M[36], double sigma2, double out[6]) {
+    double Li[6][6];  // L^-1, column by column
+    for (int c = 0; c < 6; c++) {
+        double u[6] = {0, 0, 0, 0, 0, 0}, x[6];
+        u[c] = 1.0;
+        calib_ro_lsolve6(fac + CALIB_FAC_L, u, x);
+        for (int r = 0; r < 6; r++) Li[r][c] = x[r];
+    }
+    for (int j = 0; j < 6; j++) {
+        double s = 0.0;
+        for (int k = 0; k < 6; k++) s += Li[k][j] * Li[k][j];
+        for (int k = 0; k < 6; k++)
+            for (int l = 0; l < 6; l++) s += Li[k][j] * M[6 * k + l] * Li[l][j];
+        out[j] = sqrt(s * sigma2);
+    }
+}
+
+// The step of the board coordinates: the trial board obj = obj_prev - d (d 0 for fixed coordinates), and |d|^2, |obj_prev|^2
+// in coordinate order.
+FID_HD void calib_ro_obj_trial(int n, int fixed, const double* obj_prev, const double* d, double* obj, double out[2]) {
+    double dn = 0.0, pn = 0.0;
+    for (int k = 0; k < 3 * n; k++) {
+        const double dk = calib_ro_free(k / 3, k % 3, n, fixed) ? d[k] : 0.0;
+        obj[k] = obj_prev[k] - dk;
+        dn += (obj[k] - obj_prev[k]) * (obj[k] - obj_prev[k]);
+        pn += obj_prev[k] * obj_prev[k];
+    }
+    out[0] = dn;
+    out[1] = pn;
 }
 
 }  // namespace fid

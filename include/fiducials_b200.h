@@ -699,6 +699,9 @@ int fid_map_adopt_merged(fid_map* m, int instance);
 #define FID_CALIB_E_GUESS 4      /* the guess: fx, fy <= 0, principal point outside the image, or an aspect ratio outside [0.01, 100] */
 #define FID_CALIB_E_EXTRINSICS 5 /* findExtrinsicCameraParams2 raises: non-planar view with fewer than 6 points, degenerate DLT */
 #define FID_CALIB_E_INPUT 6      /* non-finite points, bad offsets or sizes */
+#define FID_CALIB_E_RO_VIEWS 7   /* fid_calibrate_camera_ro releasing: views of different sizes or with different object points */
+#define FID_CALIB_E_RO_SINGULAR 8 /* fid_calibrate_camera_ro releasing: a non-positive pivot in the reduced system (DESIGN.md finding 21) */
+#define FID_CALIB_E_RO_RESIDUALS 9 /* fid_calibrate_camera_ro releasing: as many free parameters as residuals (2 per point) or more */
 /* cv::TermCriteria: type bit 1 = COUNT (max_iter, clamped to 1..1000; else 30), bit 2 = EPS (epsilon; else DBL_EPSILON) */
 typedef struct fid_calib_criteria {
     int32_t type;
@@ -729,6 +732,24 @@ typedef struct fid_calib_stats {
 int fid_calibrate_camera(int device, int n_views, const int32_t* offsets, const float* obj, const float* img, int width, int height, const fid_camera* guess,
                          int32_t flags, const fid_calib_criteria* criteria, fid_calib_result* result, double* rvecs, double* tvecs, double* std_extrinsics,
                          double* per_view_errors, fid_calib_stats* stats /* optional */);
+
+/* cv::calibrateCameraROExtended: fid_calibrate_camera's calibration that also re-estimates the object points (the object-releasing
+ * method of Strobl and Hirzinger), for boards whose printed geometry is not exact.  The points are released when
+ * 1 <= fixed_point <= n - 2, n the number of points of view 0; then every view must hold the same n object points (else
+ * FID_CALIB_E_RO_VIEWS), n <= FID_CALIB_RO_MAX_POINTS (else FID_CALIB_E_POINTS) and n_views <= FID_CALIB_RO_MAX_VIEWS (else
+ * FID_CALIB_E_INPUT) and fewer free parameters than residuals (else FID_CALIB_E_RO_RESIDUALS); the 3 coordinates of point 0 and of point fixed_point and z of point n - 1 stay as given, the other
+ * 3n - 7 are estimated with the camera.  Outputs besides fid_calibrate_camera's (host, optional): new_obj_points [n][3] (cv2's
+ * newObjPoints) and std_obj_points [n][3] (stdDeviationsObjPoints; exactly 0 for the fixed coordinates); *released (optional)
+ * = 1.  With fixed_point out of that range the call is fid_calibrate_camera (the same kernels and bits), *released = 0 and the
+ * object outputs are left untouched.  Device memory of a released call: about 8 (9 + 3n)^2 bytes for the reduced system,
+ * 48 (9 + 3n) min(n_views, 256) for its chunk of views and 1.6 kB per view plus 36 bytes per image point (at the caps, 1 024 points
+ * x 4 096 views: 77 + 38 + 6.6 + 151 MB, about 273 MB). */
+#define FID_CALIB_RO_MAX_POINTS 1024 /* per view, when releasing */
+#define FID_CALIB_RO_MAX_VIEWS 4096  /* when releasing */
+int fid_calibrate_camera_ro(int device, int n_views, const int32_t* offsets, const float* obj, const float* img, int width, int height, const fid_camera* guess,
+                            int32_t flags, const fid_calib_criteria* criteria, fid_calib_result* result, double* rvecs, double* tvecs, double* std_extrinsics,
+                            double* per_view_errors, fid_calib_stats* stats /* optional */, int fixed_point, float* new_obj_points, double* std_obj_points,
+                            int* released);
 
 /* ------------------------------------------------------------------------------------------------
  * JPEG ingest (NEW; SURVEY 8f-1).  Replaces the cv::imdecode that compressed_image_transport runs in front of
