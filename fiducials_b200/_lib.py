@@ -220,6 +220,16 @@ class fid_robot_pose(C.Structure):
     _fields_ = [("valid", C.c_int32), ("n_estimates", C.c_int32), ("t", C.c_double * 3), ("q", C.c_double * 4), ("variance", C.c_double)]
 
 
+class fid_ba_params(C.Structure):
+    _fields_ = [("criteria", fid_calib_criteria)]
+
+
+class fid_ba_stats(C.Structure):
+    _fields_ = [("initial_rms", C.c_double), ("final_rms", C.c_double), ("device_ms", C.c_double)] + [(k, C.c_int32) for k in (
+        "iterations", "n_steps", "frames_used", "markers_used", "observations_used", "dropped_unmapped", "dropped_duplicate", "frames_unreached", "markers_unreached",
+        "frames_init_failed", "kernel_launches", "converged")]
+
+
 class fid_map_entry(C.Structure):
     _fields_ = [("fiducial_id", C.c_int32), ("num_obs", C.c_int32)] + [(k, C.c_double) for k in ("x", "y", "z", "rx", "ry", "rz", "variance")]
 
@@ -244,7 +254,7 @@ EXPORTS = [
     "fid_map_load", "fid_map_links", "fid_map_add_links", "fid_map_update", "fid_map_update_sequence", "fid_map_update_frames", "fid_map_update_frames_async", "fid_map_sync", "fid_map_entries", "fid_map_export", "fid_map_merge", "fid_map_export_device",
     "fid_map_merge_device", "fid_map_merge_device_async", "fid_map_export_async", "fid_map_stream", "fid_map_merged_entries", "fid_map_adopt_merged", "fid_map_add_fiducial", "fid_map_refine_default_params", "fid_map_refine",
     "fid_jpeg_create", "fid_jpeg_destroy", "fid_jpeg_decode_batch", "fid_jpeg_sync", "fid_jpeg_stream", "fid_jpeg_last_stats", "fid_calibrate_camera",
-    "fid_calibrate_camera_ro",
+    "fid_calibrate_camera_ro", "fid_map_ba_default_params", "fid_map_bundle_adjust",
 ]
 
 _lib = None
@@ -348,6 +358,9 @@ def load():
     lib.fid_calibrate_camera.argtypes = [i32, i32, vp, vp, vp, i32, i32, C.POINTER(fid_camera), i32, C.POINTER(fid_calib_criteria), C.POINTER(fid_calib_result), vp, vp,
                                          vp, vp, C.POINTER(fid_calib_stats)]
     lib.fid_calibrate_camera_ro.argtypes = lib.fid_calibrate_camera.argtypes + [i32, vp, vp, C.POINTER(C.c_int)]
+    lib.fid_map_ba_default_params.argtypes = [C.POINTER(fid_ba_params)]
+    lib.fid_map_bundle_adjust.argtypes = [vp, i32, i32, vp, vp, vp, i32, C.POINTER(fid_camera), C.c_double, i32, vp, vp, C.POINTER(fid_ba_params), C.POINTER(fid_ba_stats),
+                                          vp, vp, vp, vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError if the build lost a symbol
     _lib = lib

@@ -416,6 +416,19 @@ FID_HD void calib_lm_trial_intrinsics(CalibLM* s, const double d[9]) {
     if (s->aspect != 0) s->in[0] = s->in[1] * s->aspect;
 }
 
+// CvLevMarq's (updateAlt) schedule after a trial of cost `err` from the J of cost `prev_err`, with the step's |p - pp|^2 = dn and
+// |pp|^2 = pn: a trial whose cost exceeds prev_err raises lg and is retried from the same J while lg <= 16 (false, state stays 1);
+// a kept trial lowers lg (>= -16), counts one iteration and sets state 2 after max_iter iterations or when
+// |p - pp| / (|pp| + DBL_EPSILON) < eps, else 0 (true).  Shared by the calibrations and the map bundle adjustment (map_ba.cuh).
+FID_HD bool lm_schedule_decide(int* state, int* lg, int* iters, int max_iter, double eps, double err, double prev_err, double dn, double pn) {
+    const bool keep = !(err > prev_err && ++*lg <= 16);
+    if (!keep) return false;
+    *lg = *lg - 1 > -16 ? *lg - 1 : -16;
+    ++*iters;
+    *state = (*iters >= max_iter || sqrt(dn) / (sqrt(pn) + 2.220446049250313e-16) < eps) ? 2 : 0;
+    return true;
+}
+
 // CvLevMarq's decision on a trial of cost `err` with the views' |p - pp|^2 and |pp|^2 summed in view order.
 FID_HD void calib_lm_decide(CalibLM* s, double err, double dn_views, double pn_views) {
     double dn = 0.0, pn = 0.0;
@@ -426,13 +439,9 @@ FID_HD void calib_lm_decide(CalibLM* s, double err, double dn_views, double pn_v
     dn += dn_views;
     pn += pn_views;
     s->err = err;
-    const bool keep = !(err > s->prev_err && ++s->lg <= 16);
+    const bool keep = lm_schedule_decide(&s->state, &s->lg, &s->iters, s->max_iter, s->eps, err, s->prev_err, dn, pn);
     if (s->n_steps < CALIB_MAX_STEPS) s->steps[s->n_steps] = keep ? 1 : 0;
     s->n_steps++;
-    if (!keep) return;  // state stays 1: another trial from the same J
-    s->lg = s->lg - 1 > -16 ? s->lg - 1 : -16;
-    s->iters++;
-    s->state = (s->iters >= s->max_iter || sqrt(dn) / (sqrt(pn) + 2.220446049250313e-16) < s->eps) ? 2 : 0;
 }
 
 // Stage 5, one view: the standard deviations of its rvec and tvec given S^-1 (zero rows and columns for fixed intrinsics),
@@ -536,14 +545,13 @@ FID_HD void calib_ro_ltsolve6(const double* L, const double b[6], double x[6]) {
     }
 }
 
-// One view: the Cholesky factor L of V with its diagonal times `scale`, and h = L^-1 ge (layout CALIB_FAC_*); false on a
-// non-positive pivot.
-FID_HD bool calib_ro_view_factor(const double* blk, double scale, double* fac) {
+// The Cholesky factor L (lower, packed row by row, 21) of the symmetric 6x6 matrix given by its upper triangle (21, row by row)
+// with its diagonal times `scale`; false on a non-positive pivot.
+FID_HD bool calib_chol6(const double* upper, double scale, double* L) {
     double A[6][6];
     for (int a = 0, o = 0; a < 6; a++)
-        for (int b = a; b < 6; b++, o++) A[a][b] = A[b][a] = blk[CALIB_V + o];
+        for (int b = a; b < 6; b++, o++) A[a][b] = A[b][a] = upper[o];
     for (int a = 0; a < 6; a++) A[a][a] *= scale;
-    double* L = fac + CALIB_FAC_L;
     for (int a = 0; a < 6; a++)
         for (int b = 0; b <= a; b++) {
             double s = A[a][b];
@@ -555,7 +563,14 @@ FID_HD bool calib_ro_view_factor(const double* blk, double scale, double* fac) {
                 L[a * (a + 1) / 2 + a] = sqrt(s);
             }
         }
-    calib_ro_lsolve6(L, blk + CALIB_GE, fac + CALIB_FAC_H);
+    return true;
+}
+
+// One view: the Cholesky factor L of V with its diagonal times `scale`, and h = L^-1 ge (layout CALIB_FAC_*); false on a
+// non-positive pivot.
+FID_HD bool calib_ro_view_factor(const double* blk, double scale, double* fac) {
+    if (!calib_chol6(blk + CALIB_V, scale, fac + CALIB_FAC_L)) return false;
+    calib_ro_lsolve6(fac + CALIB_FAC_L, blk + CALIB_GE, fac + CALIB_FAC_H);
     return true;
 }
 

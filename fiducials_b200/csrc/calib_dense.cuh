@@ -1,4 +1,5 @@
-// Dense FP64 kernels of fid_calibrate_camera_ro's reduced system (calib.cuh, "object release"), for sm_90a.
+// Dense FP64 kernels of the reduced systems of fid_calibrate_camera_ro (calib.cuh, "object release") and fid_map_bundle_adjust
+// (map_ba.cuh), for sm_90a.
 //
 // Matrices are row-major with a leading dimension `ld` that is a multiple of 32 (the padded size mp >= m); only the lower
 // triangle of the symmetric system is computed and read.  Every kernel sums in a fixed order and uses no atomics, so two runs
@@ -8,6 +9,7 @@
 //   k_dense_trsm   thread per row below it: the panel L21 = A21 L11^-T
 //   k_dense_trsv   CTA per right-hand side (a column of length ld): L y = x, then (backward) L^T x = y, blocked by 32
 // A blocked right-looking factorisation is potrf / trsm / syrk per 32-column panel (dense_cholesky_enqueue).
+// The kernels are static: every translation unit that includes this file (fid_calib.cu, fid_map_ba.cu) gets its own copy.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -26,7 +28,7 @@ __device__ __forceinline__ bool dense_stop(const int* status, const int* state) 
 // C[i][j] -= sum_k A(i, k) B(j, k) for the 64x64 tiles with tile row >= tile column of the n x n block C (ldc), n a multiple of
 // 32; A(i, k) = A[i * sai + k * sak], B(j, k) likewise.  Grid (ceil(n / 64), ceil(n / 64)) of 256 threads; the upper tiles return
 // at once.  A warp computes 16x32 of the tile as 2x4 mma.m8n8k4 tiles, K in steps of 16 staged in shared memory.
-__global__ void __launch_bounds__(256) k_dense_syrk(double* C, int ldc, int n, const double* A, size_t sai, size_t sak, const double* B, size_t sbj,
+static __global__ void __launch_bounds__(256) k_dense_syrk(double* C, int ldc, int n, const double* A, size_t sai, size_t sak, const double* B, size_t sbj,
                                                     size_t sbk, int K, const int* status, const int* state) {
     const int ti = blockIdx.y, tj = blockIdx.x;
     if (tj > ti || dense_stop(status, state)) return;
@@ -72,7 +74,7 @@ __global__ void __launch_bounds__(256) k_dense_syrk(double* C, int ldc, int n, c
 }
 
 // One CTA of 32 x 32 threads: the Cholesky factor of the diagonal block at (j0, j0), in place (lower).
-__global__ void __launch_bounds__(1024) k_dense_potrf(double* S, int ld, int j0, int fail_status, int* status, const int* state) {
+static __global__ void __launch_bounds__(1024) k_dense_potrf(double* S, int ld, int j0, int fail_status, int* status, const int* state) {
     if (dense_stop(status, state)) return;
     __shared__ double a[DENSE_TILE][DENSE_TILE + 1];
     __shared__ int bad;
@@ -96,7 +98,7 @@ __global__ void __launch_bounds__(1024) k_dense_potrf(double* S, int ld, int j0,
 }
 
 // Thread per row i >= j0 + 32 (below the diagonal block, up to n): L[i][j0..j0+32) = A[i][j0..j0+32) L11^-T.
-__global__ void __launch_bounds__(128) k_dense_trsm(double* S, int ld, int j0, int n, const int* status, const int* state) {
+static __global__ void __launch_bounds__(128) k_dense_trsm(double* S, int ld, int j0, int n, const int* status, const int* state) {
     if (dense_stop(status, state)) return;
     __shared__ double l[DENSE_TILE][DENSE_TILE + 1];
     for (int e = threadIdx.x; e < DENSE_TILE * DENSE_TILE; e += blockDim.x) l[e / DENSE_TILE][e % DENSE_TILE] = S[(size_t)(j0 + e / DENSE_TILE) * ld + j0 + e % DENSE_TILE];
@@ -118,7 +120,7 @@ __global__ void __launch_bounds__(128) k_dense_trsm(double* S, int ld, int j0, i
 
 // CTA per right-hand side X + b * ldx (n = the padded size, a multiple of 32): L y = x and, with `backward`, L^T x = y, in place.
 // With norms != null, norms[b] = |y|^2 (summed in row order) after the forward solve.
-__global__ void __launch_bounds__(256) k_dense_trsv(const double* L, int ld, int n, double* X, size_t ldx, int backward, double* norms, const int* status,
+static __global__ void __launch_bounds__(256) k_dense_trsv(const double* L, int ld, int n, double* X, size_t ldx, int backward, double* norms, const int* status,
                                                     const int* state) {
     if (dense_stop(status, state)) return;
     extern __shared__ double x[];
@@ -179,7 +181,7 @@ __global__ void __launch_bounds__(256) k_dense_trsv(const double* L, int ld, int
 }
 
 // Enqueue the blocked right-looking Cholesky of the n x n lower triangle of S (n a multiple of 32): 3 launches per panel.
-inline int dense_cholesky_enqueue(double* S, int n, int fail_status, int* status, const int* state, cudaStream_t st) {
+static inline int dense_cholesky_enqueue(double* S, int n, int fail_status, int* status, const int* state, cudaStream_t st) {
     int launches = 0;
     for (int j0 = 0; j0 < n; j0 += DENSE_TILE) {
         k_dense_potrf<<<1, dim3(DENSE_TILE, DENSE_TILE), 0, st>>>(S, n, j0, fail_status, status, state);

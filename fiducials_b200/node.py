@@ -1004,6 +1004,34 @@ class FiducialSlam:
         _lib.check(self.lib.fid_map_refine(self.h, instance, len(messages), off.ctypes.data_as(C.c_void_p), C.cast(arr, C.c_void_p), C.byref(p), C.byref(st)), "fid_map_refine")
         return st
 
+    def bundle_adjust(self, counts, ids, corners, K, D, fiducial_len=0.14, overrides=None, instance=0, criteria=None):
+        """fid_map_bundle_adjust: bundle adjustment of the map from recorded corners (new; DESIGN.md f16).  counts [F], ids [F][m],
+        corners [F][m][4][2] as Detector.detect_pose_batch returns them; overrides = {id: length}; criteria = cv2-style (type,
+        max_iter, epsilon) or None.  The free entries' poses are updated in place.  Returns (fid_ba_stats, rvecs [F][3],
+        tvecs [F][3], status [F], {id: standard deviations of (dtheta, dt)})."""
+        counts = np.ascontiguousarray(counts, np.int32)
+        ids = np.ascontiguousarray(ids, np.int32)
+        F, mm = ids.shape
+        corners = np.ascontiguousarray(corners, np.float32).reshape(F, mm, 8)
+        ov = dict(overrides or {})
+        ov_ids = np.ascontiguousarray(list(ov.keys()), np.int32)
+        ov_lens = np.ascontiguousarray(list(ov.values()), np.float64)
+        p = _lib.fid_ba_params()
+        _lib.check(self.lib.fid_map_ba_default_params(C.byref(p)))
+        if criteria is not None:
+            p.criteria = _lib.fid_calib_criteria(int(criteria[0]), int(criteria[1]), float(criteria[2]))
+        cam = _camera(K, D)
+        st = _lib.fid_ba_stats()
+        rv, tv, status = np.zeros((F, 3)), np.zeros((F, 3)), np.zeros(F, np.int32)
+        ents = self.entries(instance)
+        sd = np.zeros((max(len(ents), 1), 6))
+        _lib.check(self.lib.fid_map_bundle_adjust(self.h, instance, F, counts.ctypes.data_as(C.c_void_p), ids.ctypes.data_as(C.c_void_p),
+                                                  corners.ctypes.data_as(C.c_void_p), mm, C.byref(cam), float(fiducial_len), len(ov_ids),
+                                                  ov_ids.ctypes.data_as(C.c_void_p) if len(ov_ids) else None, ov_lens.ctypes.data_as(C.c_void_p) if len(ov_ids) else None,
+                                                  C.byref(p), C.byref(st), rv.ctypes.data_as(C.c_void_p), tv.ctypes.data_as(C.c_void_p),
+                                                  status.ctypes.data_as(C.c_void_p), sd.ctypes.data_as(C.c_void_p)), "fid_map_bundle_adjust")
+        return st, rv, tv, status, {e.fiducial_id: sd[k].copy() for k, e in enumerate(ents)}
+
     # multi-GPU merged view (new; SURVEY 8e): local instances are never overwritten by a merge
     def export_table(self, instance=0) -> np.ndarray:
         cap = self.p.max_fiducials

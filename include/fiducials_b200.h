@@ -752,6 +752,73 @@ int fid_calibrate_camera_ro(int device, int n_views, const int32_t* offsets, con
                             int* released);
 
 /* ------------------------------------------------------------------------------------------------
+ * Map bundle adjustment (after the calibration types it shares).
+ * ---------------------------------------------------------------------------------------------- */
+/* Bundle adjustment of a map instance from recorded marker corners (NEW -- DESIGN.md f16; the reference only folds per-marker
+ * poses, map.cpp:152-320, and fid_map_refine works from relative poses without pixels; parity stated here and pinned against
+ * scipy.optimize.least_squares on the same residuals, tests/test_hostsim_map_ba.py).
+ *   input     a recorded sequence in fid_detect_pose_batch's dense layout: counts[n_frames], ids[n_frames][max_markers],
+ *             corners[n_frames][max_markers][4][2] (float32); the camera (K, plumb_bob D); fiducial_len and the node's overrides
+ *             as fid_pose takes them
+ *   unknowns  every used frame's camera-from-map pose (R_f, t_f) (cv2's rvec / tvec convention) and every free entry's pose
+ *             T_mapFid = (R_m, t_m).  Entries with variance 0 stay fixed (the origin of autoInit / add_fiducial); none gives
+ *             FID_ERR_INVALID_ARG
+ *   residual  per observation of marker m in frame f, 8 values pi(K, D, R_f (R_m o_k + t_m) + t_f) - c_fk, k = 0..3: pi =
+ *             cv::projectPoints, o_k = getSingleMarkerObjectPoints at the marker's length (override or fiducial_len);
+ *             rms = sqrt(sum |e|^2 / corners)
+ *   counts    ids not in the map are ignored; an id seen twice in a frame drops every observation of it in that frame; frames
+ *             without a mapped marker are unused; only markers and frames connected through co-visibility to a fixed entry
+ *             take part, the others are left untouched and counted
+ *   init      per frame solvePnP(ITERATIVE) of its mapped markers as one board whose object points are the map-frame corners
+ *             narrowed to float32 (cv2.aruco.Board + matchImagePoints + cv2.solvePnP on that board), unless one marker's fid_pose
+ *             composed with its map pose reprojects the frame's corners better (candidates with a corner behind the camera
+ *             never count).  A fold's map is nearly but not
+ *             exactly planar, where solvePnP's non-planar DLT can put the camera metres off; the single-marker candidates keep
+ *             the start in the right basin.  A frame without any candidate is dropped (status 3)
+ *   solver    Levenberg-Marquardt with fid_calibrate_camera's CvLevMarq schedule, diagonals damped by 1 + lambda, the update
+ *             R <- R Exp(dtheta), t <- t + dt; every step eliminates the frames (Schur complement, dense over the free markers)
+ *             and factors the reduced system on the device.  |p| of the relative-step test = sqrt(sum angle(R)^2 + |t|^2)
+ * Output: the free entries' poses are written back in place (variances, observation counts and links are left alone; fixed
+ * and unreached entries stay byte-identical; read_only_map is not consulted).  Optional host outputs: frame_rvecs / frame_tvecs
+ * [n_frames][3] (0 for unused frames), frame_status [n_frames] (FID_BA_FRAME_*), std_entries [entries][6] in fid_map_entries
+ * order: the standard deviations of (dtheta, dt) at the optimum, sqrt(sigma^2 diag(S^-1)) with sigma^2 = sum |e|^2 /
+ * (2 corners - free parameters), 0 for fixed and unreached entries.  Device reruns are bit-identical (fixed summation orders, no
+ * atomics).  stats->converged = 0 when the run stopped at max_iter rather than on the relative-step test (the poses are still
+ * written back; the cost never rose).  Caps: FID_BA_MAX_FREE free markers, FID_BA_MAX_FRAMES frames, FID_BA_MAX_OBS
+ * observations (FID_ERR_CAPACITY above, nothing written).  FID_ERR_INVALID_ARG for non-finite corners, a bad camera, bad sizes,
+ * no fixed entry or a non-positive pivot (a pose the observations do not determine; nothing is written back then).  Waits for
+ * pending asynchronous updates first.  Device memory: about 1.3 kB per observation (including the initial poses' staging),
+ * 0.7 kB per frame, 8 bytes per pair of free markers seen together in a frame (the co-visibility lists: k markers per frame
+ * give k (k - 1) / 2 pairs) and 8 mp (mp + min(6M, 768)) bytes for the reduced system, mp = 6M rounded up to 32 (at the caps,
+ * 1 024 free markers: 302 + 38 MB, plus 5.5 GB for 2^22 observations). */
+#define FID_BA_MAX_FREE 1024
+#define FID_BA_MAX_FRAMES 65536
+#define FID_BA_MAX_OBS (1 << 22)
+#define FID_BA_FRAME_NONE 0      /* no mapped marker */
+#define FID_BA_FRAME_USED 1
+#define FID_BA_FRAME_UNREACHED 2 /* not connected to a fixed entry */
+#define FID_BA_FRAME_INIT 3      /* dropped by the initial pose (solvePnP would raise) */
+typedef struct fid_ba_params {
+    /* type bit 1 = COUNT (max_iter, clamped to 1..1000; else 100), bit 2 = EPS (epsilon on the relative step; else 1e-12) */
+    fid_calib_criteria criteria;
+} fid_ba_params;
+typedef struct fid_ba_stats {
+    double initial_rms, final_rms; /* px, at the initial poses and at the optimum */
+    double device_ms;              /* CUDA events around the device work (initial poses + solve) */
+    int32_t iterations, n_steps;   /* CvLevMarq iterations and trial steps */
+    int32_t frames_used, markers_used /* free markers solved */, observations_used;
+    int32_t dropped_unmapped, dropped_duplicate; /* detections */
+    int32_t frames_unreached, markers_unreached /* free entries not taking part */, frames_init_failed;
+    int32_t kernel_launches;
+    int32_t converged;             /* 1: the relative-step test ended the run; 0: it stopped at max_iter (poses still written back) */
+} fid_ba_stats;
+int fid_map_ba_default_params(fid_ba_params* p);
+int fid_map_bundle_adjust(fid_map* m, int instance, int n_frames, const int32_t* counts, const int32_t* ids, const float* corners, int max_markers,
+                          const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
+                          const fid_ba_params* params /* NULL = defaults */, fid_ba_stats* stats /* optional */, double* frame_rvecs, double* frame_tvecs,
+                          int32_t* frame_status, double* std_entries);
+
+/* ------------------------------------------------------------------------------------------------
  * JPEG ingest (NEW; SURVEY 8f-1).  Replaces the cv::imdecode that compressed_image_transport runs in front of
  * FiducialsNode::imageCallback (aruco_detect.cpp:332,348; default transport `compressed`,
  * aruco_detect/launch/aruco_detect.launch:6,28).  The Huffman bit stream of every image is decoded on host threads
