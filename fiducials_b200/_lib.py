@@ -230,6 +230,12 @@ class fid_ba_stats(C.Structure):
         "frames_init_failed", "kernel_launches", "converged")]
 
 
+class fid_localization(C.Structure):
+    _fields_ = [(k, C.c_int32) for k in ("status", "n_markers", "n_points", "lm_iters", "start", "have_base", "cov_ok")] + [
+        ("rvec", C.c_double * 3), ("tvec", C.c_double * 3), ("t", C.c_double * 3), ("q", C.c_double * 4), ("image_error", C.c_double), ("object_error", C.c_double),
+        ("sigma2", C.c_double), ("covariance", C.c_double * 36)]
+
+
 class fid_map_entry(C.Structure):
     _fields_ = [("fiducial_id", C.c_int32), ("num_obs", C.c_int32)] + [(k, C.c_double) for k in ("x", "y", "z", "rx", "ry", "rz", "variance")]
 
@@ -254,7 +260,7 @@ EXPORTS = [
     "fid_map_load", "fid_map_links", "fid_map_add_links", "fid_map_update", "fid_map_update_sequence", "fid_map_update_frames", "fid_map_update_frames_async", "fid_map_sync", "fid_map_entries", "fid_map_export", "fid_map_merge", "fid_map_export_device",
     "fid_map_merge_device", "fid_map_merge_device_async", "fid_map_export_async", "fid_map_stream", "fid_map_merged_entries", "fid_map_adopt_merged", "fid_map_add_fiducial", "fid_map_refine_default_params", "fid_map_refine",
     "fid_jpeg_create", "fid_jpeg_destroy", "fid_jpeg_decode_batch", "fid_jpeg_sync", "fid_jpeg_stream", "fid_jpeg_last_stats", "fid_calibrate_camera",
-    "fid_calibrate_camera_ro", "fid_map_ba_default_params", "fid_map_bundle_adjust",
+    "fid_calibrate_camera_ro", "fid_map_ba_default_params", "fid_map_bundle_adjust", "fid_map_localize",
 ]
 
 _lib = None
@@ -361,6 +367,8 @@ def load():
     lib.fid_map_ba_default_params.argtypes = [C.POINTER(fid_ba_params)]
     lib.fid_map_bundle_adjust.argtypes = [vp, i32, i32, vp, vp, vp, i32, C.POINTER(fid_camera), C.c_double, i32, vp, vp, C.POINTER(fid_ba_params), C.POINTER(fid_ba_stats),
                                           vp, vp, vp, vp]
+    lib.fid_map_localize.argtypes = [vp, i32, i32, vp, vp, vp, i32, C.POINTER(fid_camera), C.c_double, i32, vp, vp, C.c_double, C.POINTER(fid_tf),
+                                     C.POINTER(fid_localization)]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError if the build lost a symbol
     _lib = lib

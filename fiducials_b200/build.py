@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libfiducials_b200.so")
-SOURCES = ["fid_api.cu", "fid_map.cu", "fid_map_refine.cu", "fid_map_ba.cu", "fid_jpeg.cu", "fid_calib.cu"]
+SOURCES = ["fid_api.cu", "fid_map.cu", "fid_map_refine.cu", "fid_map_ba.cu", "fid_map_localize.cu", "fid_jpeg.cu", "fid_calib.cu"]
 # --fmad=false: OpenCV's float32/float64 arithmetic (cornerSubPix, perimeters, the LM trajectory) is
 # compiled without FMA contraction on x86-64; contracting here would change iteration counts.
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "--fmad=false", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]

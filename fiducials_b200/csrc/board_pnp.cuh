@@ -248,6 +248,82 @@ FID_HD bool board_homography(int n, const Pts& pts, double Hm[9]) {
     return true;
 }
 
+// The sum of squared reprojection errors of the n points obj / img at p = {rvec, tvec}; f32: with the projections rounded to float
+// (getReprojectionError).
+FID_HD double board_sq_error(int n, const float* obj, const float* img, const Camera& cam, const double p[6], bool f32) {
+    double R[9], s[1];
+    rodrigues_v2m(p, R, nullptr);
+    board_sum<1>(n, [&](int i, double v[1]) {
+        double uv[2];
+        project_point(obj[3 * i], obj[3 * i + 1], obj[3 * i + 2], R, nullptr, p, cam, uv, nullptr);
+        if (f32) {
+            const double e = dist2f(img[2 * i], img[2 * i + 1], (float)uv[0], (float)uv[1]);
+            v[0] = e * e;
+        } else {
+            const double ex = uv[0] - img[2 * i], ey = uv[1] - img[2 * i + 1];
+            v[0] = ex * ex + ey * ey;
+        }
+    }, s);
+    return s[0];
+}
+
+// Step 4 of solvePnP(ITERATIVE) (cv::findExtrinsicCameraParams2's refinement; also all that solvePnP runs with
+// useExtrinsicGuess): Levenberg-Marquardt on the distorted reprojection error of the n points from p = {rvec, tvec} (updated in
+// place), the CvLevMarq schedule of pnp.cuh (<= 20 iterations, FLT_EPSILON relative step).  Returns the iterations.
+FID_HD int board_pose_lm(int n, const float* obj, const float* img, const Camera& cam, double p[6]) {
+    auto normal_eq = [&](const double q[6], double JtJ[6][6], double JtE[6], double* err2) {
+        double R[9], dRdr[27], s[28];
+        rodrigues_v2m(q, R, dRdr);
+        board_sum<28>(n, [&](int i, double v[28]) {
+            double uv[2], J[2][6];
+            project_point(obj[3 * i], obj[3 * i + 1], obj[3 * i + 2], R, dRdr, q, cam, uv, J);
+            const double ex = uv[0] - img[2 * i], ey = uv[1] - img[2 * i + 1];
+            int o = 0;
+            for (int a = 0; a < 6; a++)
+                for (int b = a; b < 6; b++) v[o++] = J[0][a] * J[0][b] + J[1][a] * J[1][b];
+            for (int a = 0; a < 6; a++) v[21 + a] = J[0][a] * ex + J[1][a] * ey;
+            v[27] = ex * ex + ey * ey;
+        }, s);
+        for (int a = 0, o = 0; a < 6; a++)
+            for (int b = a; b < 6; b++, o++) JtJ[a][b] = JtJ[b][a] = s[o];
+        for (int a = 0; a < 6; a++) JtE[a] = s[21 + a];
+        *err2 = s[27];
+    };
+    double JtJ[6][6], JtE[6], e2;
+    normal_eq(p, JtJ, JtE, &e2);
+    int lam = -3, iters = 0;
+    double prev_err = sqrt(e2), en = 0.0;
+    for (;;) {
+        double prev[6];
+        for (int a = 0; a < 6; a++) prev[a] = p[a];
+        for (;;) {
+            double A[6][6], delta[6];
+            const double scale = 1.0 + exp(lam * 2.302585092994046);
+            for (int a = 0; a < 6; a++)
+                for (int b = 0; b < 6; b++) A[a][b] = a == b ? JtJ[a][b] * scale : JtJ[a][b];
+            solve_sym6(A, JtE, delta);
+            for (int a = 0; a < 6; a++) p[a] = prev[a] - delta[a];
+            en = sqrt(board_sq_error(n, obj, img, cam, p, false));
+            if (en > prev_err) {
+                lam++;
+                if (lam <= 16) continue;
+            }
+            break;
+        }
+        lam = lam - 1 > -16 ? lam - 1 : -16;
+        iters++;
+        double dn = 0.0, pn = 0.0;
+        for (int a = 0; a < 6; a++) {
+            dn += (p[a] - prev[a]) * (p[a] - prev[a]);
+            pn += prev[a] * prev[a];
+        }
+        if (iters >= 20 || sqrt(dn) / sqrt(pn) < 1.1920928955078125e-07) break;
+        prev_err = en;
+        normal_eq(p, JtJ, JtE, &e2);
+    }
+    return iters;
+}
+
 // solvePnP(ITERATIVE) of n matched points: obj [n][3] float32 (metres), img [n][2] float32 (px); mn [n][2] is scratch for the
 // normalised points (each lane writes and reads only its own points).  Fills everything of out but n_markers.
 FID_HD void solve_board_pose(int n, const float* obj, const float* img, double* mn, const Camera& cam, BoardPoseOut* out) {
@@ -384,73 +460,7 @@ FID_HD void solve_board_pose(int n, const float* obj, const float* img, double* 
         rodrigues_m2v(Rm, p);
     }
     // 4. Levenberg-Marquardt (CvLevMarq schedule, as solve_marker_pose)
-    auto normal_eq = [&](const double q[6], double JtJ[6][6], double JtE[6], double* err2) {
-        double R[9], dRdr[27], s[28];
-        rodrigues_v2m(q, R, dRdr);
-        board_sum<28>(n, [&](int i, double v[28]) {
-            double uv[2], J[2][6];
-            project_point(obj[3 * i], obj[3 * i + 1], obj[3 * i + 2], R, dRdr, q, cam, uv, J);
-            const double ex = uv[0] - img[2 * i], ey = uv[1] - img[2 * i + 1];
-            int o = 0;
-            for (int a = 0; a < 6; a++)
-                for (int b = a; b < 6; b++) v[o++] = J[0][a] * J[0][b] + J[1][a] * J[1][b];
-            for (int a = 0; a < 6; a++) v[21 + a] = J[0][a] * ex + J[1][a] * ey;
-            v[27] = ex * ex + ey * ey;
-        }, s);
-        for (int a = 0, o = 0; a < 6; a++)
-            for (int b = a; b < 6; b++, o++) JtJ[a][b] = JtJ[b][a] = s[o];
-        for (int a = 0; a < 6; a++) JtE[a] = s[21 + a];
-        *err2 = s[27];
-    };
-    auto sq_error = [&](const double q[6], bool f32) {
-        // sum of squared reprojection errors; f32: with the projections rounded to float (getReprojectionError)
-        double R[9], s[1];
-        rodrigues_v2m(q, R, nullptr);
-        board_sum<1>(n, [&](int i, double v[1]) {
-            double uv[2];
-            project_point(obj[3 * i], obj[3 * i + 1], obj[3 * i + 2], R, nullptr, q, cam, uv, nullptr);
-            if (f32) {
-                const double e = dist2f(img[2 * i], img[2 * i + 1], (float)uv[0], (float)uv[1]);
-                v[0] = e * e;
-            } else {
-                const double ex = uv[0] - img[2 * i], ey = uv[1] - img[2 * i + 1];
-                v[0] = ex * ex + ey * ey;
-            }
-        }, s);
-        return s[0];
-    };
-    double JtJ[6][6], JtE[6], e2;
-    normal_eq(p, JtJ, JtE, &e2);
-    int lam = -3, iters = 0;
-    double prev_err = sqrt(e2), en = 0.0;
-    for (;;) {
-        double prev[6];
-        for (int a = 0; a < 6; a++) prev[a] = p[a];
-        for (;;) {
-            double A[6][6], delta[6];
-            const double scale = 1.0 + exp(lam * 2.302585092994046);
-            for (int a = 0; a < 6; a++)
-                for (int b = 0; b < 6; b++) A[a][b] = a == b ? JtJ[a][b] * scale : JtJ[a][b];
-            solve_sym6(A, JtE, delta);
-            for (int a = 0; a < 6; a++) p[a] = prev[a] - delta[a];
-            en = sqrt(sq_error(p, false));
-            if (en > prev_err) {
-                lam++;
-                if (lam <= 16) continue;
-            }
-            break;
-        }
-        lam = lam - 1 > -16 ? lam - 1 : -16;
-        iters++;
-        double dn = 0.0, pn = 0.0;
-        for (int a = 0; a < 6; a++) {
-            dn += (p[a] - prev[a]) * (p[a] - prev[a]);
-            pn += prev[a] * prev[a];
-        }
-        if (iters >= 20 || sqrt(dn) / sqrt(pn) < 1.1920928955078125e-07) break;
-        prev_err = en;
-        normal_eq(p, JtJ, JtE, &e2);
-    }
+    const int iters = board_pose_lm(n, obj, img, cam, p);
     out->status = 1;
     out->lm_iters = iters;
     for (int k = 0; k < 3; k++) {
@@ -458,7 +468,7 @@ FID_HD void solve_board_pose(int n, const float* obj, const float* img, double* 
         out->tvec[k] = p[3 + k];
     }
     // reprojection error with the projections rounded to float32 (getReprojectionError :208-219, over all matched points)
-    out->image_error = sq_error(p, true) / n;
+    out->image_error = board_sq_error(n, obj, img, cam, p, true) / n;
     // quaternion (:447-448)
     const double angle = sqrt(p[0] * p[0] + p[1] * p[1] + p[2] * p[2]);
     const double ax = p[0] / angle, ay = p[1] / angle, az = p[2] / angle;

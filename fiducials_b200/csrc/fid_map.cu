@@ -305,7 +305,7 @@ extern "C" int fid_map_destroy(fid_map* m) {
     if (!m) return FID_ERR_INVALID_ARG;
     cudaSetDevice(m->device);
     cudaDeviceSynchronize();
-    void* ptrs[] = {m->d_var_scratch, m->d_slot_scratch, m->d_merged, m->d_merged_hdr, m->d_hash, m->d_state, m->d_entries, m->d_links, m->d_export, m->d_obs, m->d_offsets, m->d_robot, m->d_tf, m->d_merge_in};
+    void* ptrs[] = {m->d_var_scratch, m->d_slot_scratch, m->d_merged, m->d_merged_hdr, m->d_hash, m->d_state, m->d_entries, m->d_links, m->d_export, m->d_obs, m->d_offsets, m->d_robot, m->d_tf, m->d_merge_in, m->d_loc};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (m->stream) cudaStreamDestroy(m->stream);

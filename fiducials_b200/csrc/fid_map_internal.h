@@ -42,5 +42,7 @@ struct fid_map {
     size_t merge_cap = 0;
     fid::MapEntry* d_merged = nullptr;     // [cap] merged view (ids ascending)
     struct MergedHeader* d_merged_hdr = nullptr;
+    char* d_loc = nullptr;                 // fid_map_localize: inputs, per-frame scratch and results (grown by the call)
+    size_t loc_cap = 0;
 };
 

@@ -189,9 +189,11 @@ FID_HD double ba_reproj(int n, const float* obj, const float* img, const Camera&
 // A frame's initial pose (see the top of this file): n markers, obj [n][4][3] their map-frame corners (float32), img [n][4][2]
 // their corners, mn [4n][2] scratch, len_f [n] their lengths as fid_pose narrows them, mpose [n][12] their map poses.  Device:
 // called by the 32 lanes of a warp together (every lane computes the same bits).  False when no candidate has every corner in
-// front of the camera and a finite error.
-FID_HD bool ba_init_frame(int n, const float* obj, const float* img, double* mn, const Camera& cam, const float* len_f, const double* mpose, double pose[12]) {
+// front of the camera and a finite error.  start (optional): 0 when the board pose was taken, 1 + j for marker j's own pose.
+FID_HD bool ba_init_frame(int n, const float* obj, const float* img, double* mn, const Camera& cam, const float* len_f, const double* mpose, double pose[12],
+                          int* start = nullptr) {
     double eb = -1.0, ec = -1.0, cand[12], bpose[12];
+    int jc = -1;
     BoardPoseOut bo;
     solve_board_pose(4 * n, obj, img, mn, cam, &bo);
     if (bo.status == 1) {
@@ -213,12 +215,15 @@ FID_HD bool ba_init_frame(int n, const float* obj, const float* img, double* mn,
         const double e = ba_reproj(4 * n, obj, img, cam, cand);
         if (e >= 0.0 && e < 1e300 && (ec < 0.0 || e < ec)) {
             ec = e;
+            jc = j;
             for (int k = 0; k < 12; k++) pose[k] = cand[k];
         }
     }
     // the board pose (cv2's) unless a marker's pose reprojects the frame's corners better
-    if (eb >= 0.0 && !(ec >= 0.0 && ec < eb))
+    const bool board = eb >= 0.0 && !(ec >= 0.0 && ec < eb);
+    if (board)
         for (int k = 0; k < 12; k++) pose[k] = bpose[k];
+    if (start) *start = board ? 0 : 1 + jc;
     return eb >= 0.0 || ec >= 0.0;
 }
 
@@ -419,7 +424,7 @@ inline void ba_plan_solve(int n_slots, const uint8_t* fixed, const uint8_t* init
 }
 
 // The marker length of an id: its override, else fiducial_len.
-inline double ba_marker_len(int32_t id, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens) {
+FID_HD double ba_marker_len(int32_t id, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens) {
     for (int k = 0; k < n_override; k++)
         if (override_ids[k] == id) return override_lens[k];
     return fiducial_len;

@@ -349,6 +349,48 @@ class FiducialSlam {
         return Transform{t[0], t[1], t[2], q[0], q[1], q[2], q[3]};
     }
 
+    // ---- localization against the map (new, no reference counterpart; fid_map_localize) ----
+    // The /fiducial_vertices message (aruco_detect.cpp:358-379: ids and the float32 corners as float64) and the latched CameraInfo
+    // (K, first five plumb_bob D) give the camera pose that all visible mapped markers determine together, with its covariance.
+    // fiducial_len / overrides as the detector node uses them; T_camBase = the tf lookup camera -> base (nullptr: the camera's pose).
+    fid_localization localize(const FiducialArray& vertices, const fid_camera& cam, double fiducial_len, const std::map<int, double>& overrides,
+                              const fid_tf* T_camBase, double max_entry_variance = -1.0) {
+        const int n = (int)vertices.fiducials.size();
+        std::vector<int32_t> ids(std::max(n, 1), -1);
+        std::vector<float> corners(8 * (size_t)std::max(n, 1), 0.f);
+        for (int i = 0; i < n; i++) {
+            const Fiducial& v = vertices.fiducials[i];
+            ids[i] = v.fiducial_id;
+            const double c[8] = {v.x0, v.y0, v.x1, v.y1, v.x2, v.y2, v.x3, v.y3};
+            for (int k = 0; k < 8; k++) corners[8 * (size_t)i + k] = (float)c[k];
+        }
+        std::vector<int32_t> ov_ids;
+        std::vector<double> ov_lens;
+        for (const auto& kv : overrides) {
+            ov_ids.push_back(kv.first);
+            ov_lens.push_back(kv.second);
+        }
+        const int32_t count = n;
+        fid_localization out;
+        check(fid_map_localize(map, 0, 1, &count, ids.data(), corners.data(), std::max(n, 1), &cam, fiducial_len, (int)ov_ids.size(), ov_ids.data(), ov_lens.data(),
+                               max_entry_variance, T_camBase, &out),
+              "fid_map_localize");
+        return out;
+    }
+    double multiErrorThreshold = -1.0;  // rosparam multi_error_theshold, map.cpp:127-129 (-1: never switches)
+    // What goes on /fiducial_pose: the joint pose and its covariance when multiErrorThreshold >= 0, loc->status == FID_LOC_POSE and
+    // loc->object_error < multiErrorThreshold; otherwise the fold's pose with robotPoseCovariance.  covariance_diagonal overrides
+    // the diagonal of either (map.cpp:341-345).  Publication only: the fold and the map are unchanged.
+    Transform publishedPose(const fid_robot_pose& robot, const fid_localization* loc, double cov[36]) const {
+        if (loc && multiErrorThreshold >= 0 && loc->status == FID_LOC_POSE && loc->object_error < multiErrorThreshold) {
+            for (int i = 0; i < 36; i++) cov[i] = loc->covariance[i];
+            for (int i = 0; overridePublishedCovariance && i < 6; i++) cov[i * 6 + i] = covarianceDiagonal[i];
+            return Transform{loc->t[0], loc->t[1], loc->t[2], loc->q[0], loc->q[1], loc->q[2], loc->q[3]};
+        }
+        robotPoseCovariance(robot, cov);
+        return Transform{robot.t[0], robot.t[1], robot.t[2], robot.q[0], robot.q[1], robot.q[2], robot.q[3]};
+    }
+
     // publishMap, map.cpp:629-654
     FiducialMapEntryArray publishMap() {
         std::vector<fid_map_entry> e(cap);

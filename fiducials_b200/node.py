@@ -1032,6 +1032,48 @@ class FiducialSlam:
                                                   status.ctypes.data_as(C.c_void_p), sd.ctypes.data_as(C.c_void_p)), "fid_map_bundle_adjust")
         return st, rv, tv, status, {e.fiducial_id: sd[k].copy() for k, e in enumerate(ents)}
 
+    LOCALIZATION_DTYPE = np.dtype(_lib.fid_localization)
+
+    def localize(self, counts, ids, corners, K, D, fiducial_len=0.14, overrides=None, T_camBase=None, instance=0, max_entry_variance=-1):
+        """fid_map_localize: per frame, the camera pose that every visible mapped marker's corners determine together, with its
+        covariance (new; DESIGN.md f17).  counts [F], ids [F][m], corners [F][m][4][2] as Detector.detect_pose_batch returns them;
+        overrides = {id: length}; T_camBase = 7-vector (x y z qx qy qz qw) of the camera mount, or None for the camera's own pose;
+        max_entry_variance >= 0 leaves out entries less certain than that.  The map is not changed.  Returns a LOCALIZATION_DTYPE
+        array [F] (status 1 pose, 0 no usable mapped marker, -1 no start)."""
+        counts = np.ascontiguousarray(counts, np.int32)
+        ids = np.ascontiguousarray(ids, np.int32)
+        F, mm = ids.shape
+        corners = np.ascontiguousarray(corners, np.float32).reshape(F, mm, 8)
+        ov = dict(overrides or {})
+        ov_ids = np.ascontiguousarray(list(ov.keys()), np.int32)
+        ov_lens = np.ascontiguousarray(list(ov.values()), np.float64)
+        cam = _camera(K, D)
+        cb = _tf(T_camBase)
+        out = np.zeros(F, self.LOCALIZATION_DTYPE)
+        _lib.check(self.lib.fid_map_localize(self.h, instance, F, counts.ctypes.data_as(C.c_void_p), ids.ctypes.data_as(C.c_void_p), corners.ctypes.data_as(C.c_void_p),
+                                             mm, C.byref(cam), float(fiducial_len), len(ov_ids), ov_ids.ctypes.data_as(C.c_void_p) if len(ov_ids) else None,
+                                             ov_lens.ctypes.data_as(C.c_void_p) if len(ov_ids) else None, float(max_entry_variance),
+                                             C.byref(cb) if cb is not None else None, out.ctypes.data_as(C.POINTER(_lib.fid_localization))), "fid_map_localize")
+        return out
+
+    # multi_error_theshold (map.cpp:127-129; its default -1 never switches): the object error below which /fiducial_pose carries
+    # the joint pose of localize() instead of the fold's
+    multi_error_threshold = -1.0
+
+    def published_pose(self, robot, loc=None):
+        """What goes on /fiducial_pose: (t[3], q_xyzw[4], covariance[36]).  The joint pose of a localize() record and its
+        covariance when multi_error_threshold >= 0, loc's status is 1 and its object_error is below the threshold; otherwise the
+        fold's robot pose with robotPoseCovariance.  covariance_diagonal overrides the diagonal of either (map.cpp:341-345).
+        Publication only: the fold and the map are unchanged."""
+        if loc is not None and self.multi_error_threshold >= 0 and int(loc["status"]) == 1 and float(loc["object_error"]) < self.multi_error_threshold:
+            cov = [float(v) for v in loc["covariance"]]
+            d = self.covariance_diagonal
+            if d is not None and len(d) == 6 and all(v != 0 for v in d):
+                for i in range(6):
+                    cov[i * 6 + i] = float(d[i])
+            return [float(v) for v in loc["t"]], [float(v) for v in loc["q"]], cov
+        return list(robot.t[:]), list(robot.q[:]), self.robotPoseCovariance(robot)
+
     # multi-GPU merged view (new; SURVEY 8e): local instances are never overwritten by a merge
     def export_table(self, instance=0) -> np.ndarray:
         cap = self.p.max_fiducials

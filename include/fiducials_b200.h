@@ -818,6 +818,41 @@ int fid_map_bundle_adjust(fid_map* m, int instance, int n_frames, const int32_t*
                           const fid_ba_params* params /* NULL = defaults */, fid_ba_stats* stats /* optional */, double* frame_rvecs, double* frame_tvecs,
                           int32_t* frame_status, double* std_entries);
 
+/* Localization against the map: one camera pose per frame from every visible mapped marker's corners together, with its
+ * covariance (NEW -- DESIGN.md f17; the reference's updatePose, map.cpp:247-391, averages one pose per marker with heuristic
+ * variances, and the `multi_error_theshold` it reads at :127-129 for a multi-fiducial pose is never used; stated here and pinned
+ * against cv2, tests/test_hostsim_map_localize.py).  Per frame f of the dense fid_detect_pose_batch layout (counts, ids, corners):
+ *   match     a detection counts when its id is in the map instance, appears once in the frame, and (max_entry_variance >= 0)
+ *             the entry's variance is <= max_entry_variance; detection order is kept
+ *   board     each counted marker's getSingleMarkerObjectPoints at its length (override or fiducial_len) through its entry's
+ *             pose, narrowed to float32: the cv2.aruco.Board of the map's markers
+ *   start     fid_map_bundle_adjust's initial pose: the board's solvePnP(ITERATIVE), unless one marker's own fid_pose composed
+ *             with its map pose reprojects all the frame's corners better (candidates with a corner behind the camera never
+ *             count).  start = 0 (board) or 1 + k (the k-th counted marker); none: status FID_LOC_NO_START
+ *   LM        cv2.solvePnP(obj, img, K, D, rvec0, tvec0, useExtrinsicGuess=True, SOLVEPNP_ITERATIVE) from that start: rvec, tvec
+ *             (camera-from-map), lm_iters; image_error = mean squared reprojection error with float32-rounded projections
+ *   pose      t, q (x y z w): T_mapBase = T_mapCam T_camBase when T_camBase is given (have_base = 1; updatePose's composition,
+ *             map.cpp:284), else T_mapCam
+ *   cov       row-major 6x6 over (x, y, z, rotation about map X, Y, Z) of that pose (ROS PoseWithCovariance order) for the
+ *             perturbation (Exp([dtheta]x) R, t + dt): sigma2 (J^T J)^-1, J the Jacobian of every corner residual at the final
+ *             pose, sigma2 = sum |e|^2 / (2 n_points - 6); cov_ok = 0 and a zero covariance on a non-positive Cholesky pivot
+ *   object_error  (image_error / mean |c0 - c2| px) (mean |marker centre in the camera frame| / fiducial_len) over the counted
+ *             markers: aruco_detect.cpp:493-495's formula at the joint pose, the quantity multi_error_theshold is compared with
+ * out[n_frames].  FID_ERR_INVALID_ARG for a bad camera, non-finite corners, counts[f] outside 0..max_markers, max_markers outside
+ * 1..FID_MAX_MARKERS, non-positive lengths or a bad instance; FID_ERR_CAPACITY above FID_BA_MAX_FRAMES frames; nothing is
+ * written then.  The map is not changed.  Runs on the map's stream after pending asynchronous updates; device reruns are
+ * bit-identical (a warp per frame, fixed summation orders, no atomics). */
+#define FID_LOC_POSE 1
+#define FID_LOC_NONE 0      /* no usable mapped marker */
+#define FID_LOC_NO_START (-1)
+typedef struct fid_localization {
+    int32_t status, n_markers, n_points, lm_iters, start, have_base, cov_ok;
+    double rvec[3], tvec[3], t[3], q[4], image_error, object_error, sigma2, covariance[36];
+} fid_localization;
+int fid_map_localize(fid_map* m, int instance, int n_frames, const int32_t* counts, const int32_t* ids, const float* corners, int max_markers,
+                     const fid_camera* cam, double fiducial_len, int n_override, const int32_t* override_ids, const double* override_lens,
+                     double max_entry_variance, const fid_tf* T_camBase /* NULL: camera pose only */, fid_localization* out /* [n_frames] */);
+
 /* ------------------------------------------------------------------------------------------------
  * JPEG ingest (NEW; SURVEY 8f-1).  Replaces the cv::imdecode that compressed_image_transport runs in front of
  * FiducialsNode::imageCallback (aruco_detect.cpp:332,348; default transport `compressed`,
